@@ -194,6 +194,9 @@ struct gpbdev_vecchia {
   bool stored_latent = false, last_latent = false;
   double stored_var = 0., stored_range = 0., last_var = 0., last_range = 0.;
   int knn_replayed = 0;  // queries whose neighbour set was re-derived by the exact replay of the reference walk
+  // kernel switches, read from the environment when the engine is created (gpbdev_vecchia_create)
+  bool grad_stores = true;  // GPB200_GRAD_STORES=0: no STORE shortcut after a gradient pass, no extra stores in that pass
+  bool nll1_only = false;   // GPB200_NLL_KERNEL=1: one-observation kernel also at d = 2, 20 < m <= 30
   std::vector<int32_t> nn_host;  // kept for the lazy CSC build
 };
 
@@ -251,7 +254,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
   // GPBoost iteration: OptimCovPar's last accepted trial was a gradient pass at the final parameters on this response, and
   // CalcGradient asks for the factor at the same state right after (regression_objective.hpp:164-165): nothing to recompute.
   // GPB200_GRAD_STORES=0 switches the shortcut (and the extra stores of the gradient pass) off.
-  static const bool grad_stores = []() { const char* e = std::getenv("GPB200_GRAD_STORES"); return !(e && std::string(e) == "0"); }();
+  const bool grad_stores = h->grad_stores;
   if (mode == gpb::MODE_STORE && !latent && grad_stores && h->factor_stored && h->stored_cov == cov_type && h->stored_latent == latent &&
       h->stored_var == var && h->stored_range == range && h->last_cov == cov_type && h->last_latent == latent && h->last_var == var &&
       h->last_range == range)
@@ -308,8 +311,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
   }
   // likelihood and gradient passes at the headline shape (d = 2, 20 < m <= 30): two observations per warp (vecchia_nll2.cuh);
   // GPB200_NLL_KERNEL=1 keeps the one-observation kernel
-  static const bool nll1_only = []() { const char* e = std::getenv("GPB200_NLL_KERNEL"); return e && std::string(e) == "1"; }();
-  if ((mode == gpb::MODE_NLL || mode == gpb::MODE_STORE || (mode == gpb::MODE_GRAD && !latent)) && h->d == 2 && h->m > 20 && !nll1_only) {
+  if ((mode == gpb::MODE_NLL || mode == gpb::MODE_STORE || (mode == gpb::MODE_GRAD && !latent)) && h->d == 2 && h->m > 20 && !h->nll1_only) {
     FactorKernel k2 = nullptr;
 #define GPB_PICK2(COVID)                                                                                                              \
     k2 = mode == gpb::MODE_NLL ? gpb::vecchia_nll2_kernel<COVID, gpb::MODE_NLL>                                                      \
@@ -397,6 +399,8 @@ int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, i
   CUDA_TRY(cudaSetDevice(device));
   gpbdev_vecchia* h = new gpbdev_vecchia();
   h->device = device; h->n = n; h->d = d; h->m = m; h->row_begin = row_begin; h->row_end = row_end;
+  if (const char* e = std::getenv("GPB200_GRAD_STORES")) h->grad_stores = std::string(e) != "0";
+  if (const char* e = std::getenv("GPB200_NLL_KERNEL")) h->nll1_only = std::string(e) == "1";
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;

@@ -75,11 +75,12 @@ def r_binary_test_data():
     return coords, (sim_rand_unif(n, 0.2341) < probs).astype(np.float64)
 
 
-def binary_synth(n, seed=1, with_offset=False):
-    """Synthetic coords U[0,1]^2, a smooth latent surface and Bernoulli(logit) labels; optional fixed-effect offset."""
+def binary_synth(n, seed=1, with_offset=False, d=2):
+    """Synthetic coords U[0,1]^d, a smooth latent surface and Bernoulli(logit) labels; optional fixed-effect offset.
+    The surface depends on the first and the last coordinate; at d = 2 these are the data the Laplace goldens were made from."""
     rng = np.random.default_rng(seed)
-    coords = rng.random((n, 2))
-    latent = 1.5 * np.sin(6 * coords[:, 0]) * np.cos(4 * coords[:, 1]) + 0.3 * rng.standard_normal(n)
+    coords = rng.random((n, d))
+    latent = 1.5 * np.sin(6 * coords[:, 0]) * np.cos(4 * coords[:, -1]) + 0.3 * rng.standard_normal(n)
     offset = 0.5 * np.cos(3 * coords[:, 0]) - 0.2 if with_offset else None
     eta = latent + (offset if with_offset else 0.)
     y = (rng.random(n) < 1. / (1. + np.exp(-eta))).astype(np.float64)
