@@ -284,8 +284,8 @@ __global__ void __launch_bounds__(kHistMaxWarps * 32, 1) hist2_kernel(const uint
 
 // hist3_kernel = hist2_kernel with the two shared-memory savings its ncu capture asks for:
 // tile rows padded by 8 bytes (the four 8-byte bin words of a warp fall into different banks: 2 wavefronts instead of 8) and the
-// step's gradients loaded only by leaders whose group has later members. NOT COVERED BY THE TESTS (written after the round's
-// GPU budget was spent): opt-in with GPB200_HIST_KERNEL=3, not part of the parity tests until it has passed them once.
+// step's gradients loaded only by leaders whose group has later members. The default (GPB200_HIST_KERNEL=3; 4 = the PLAIN_COUNT
+// form); tests/test_tree_kernels_gpu.py runs both in every leaf loop.
 constexpr int kHist3Stride = kHistTile + 8;
 static inline size_t hist3_smem(int nw) { return (size_t)nw * 4 * kBins * 12 + 64 * kHist3Stride + kHistTile * 8; }
 // PLAIN_COUNT: the leader updates the integer counter with an ordinary load / add / store like the gradient sum (it is the only lane
@@ -695,8 +695,7 @@ __global__ void __launch_bounds__(kFusedSlices * kBins) reduce_scan_kernel(
 }
 
 // reduce_scan2_kernel = reduce_scan_kernel with the gains of the thresholds evaluated by one thread each (the two fp64 divisions
-// per threshold are paid once instead of eight times per lane).
-// NOT COVERED BY THE TESTS: opt-in with GPB200_FUSED_SCAN=2.
+// per threshold are paid once instead of eight times per lane). The default (GPB200_FUSED_SCAN=2).
 // counts + sequential running sums of one child: the first half of scan_feature
 __device__ __forceinline__ void scan_sums(const double* h, int nb, const LeafArgs& a, int lane, ScanScratch* scr) {
   double* rsg = scr->rsg;
@@ -1291,7 +1290,7 @@ struct gpbdev_tree {
   const double* graph_grad = nullptr;
   double graph_hess = 0.;
   // Implementation switches (environment, read at creation; every combination below passes the same parity tests,
-  // tests/test_tree_gpu.py::test_tree_kernel_variants_match_oracle). Defaults = the fastest verified set.
+  // tests/test_tree_kernels_gpu.py runs every combination against the oracle). Defaults = the fastest verified set.
   int device_loop = 2;             // GPB200_TREE_LOOP = graph (2, default) | device (1) | host (0). Row-sharded learners use the host loop.
   TreeDevState* state_dev = nullptr;
   TreeDevState* state_host = nullptr;  // pinned
@@ -1361,6 +1360,7 @@ static int tree_create_common(gpbdev_tree_t* out, int device, int64_t n, int F, 
   if (!out || (!bins_feature_major && !bins_dev) || !num_bin || !cfg) return tfail("gpbdev_tree_create: null argument");
   if (n <= 0 || F <= 0) return tfail("gpbdev_tree_create: need n > 0 and F > 0");
   if (cfg->num_leaves < 2) return tfail("gpbdev_tree_create: num_leaves must be >= 2");
+  if (cfg->min_data_in_leaf < 0) return tfail("gpbdev_tree_create: min_data_in_leaf must be >= 0");
   for (int f = 0; f < F; ++f)
     if (num_bin[f] < 1 || num_bin[f] > kBins) return tfail("gpbdev_tree_create: num_bin must be in [1, 256]");
   int ndev = 0;
@@ -1371,6 +1371,10 @@ static int tree_create_common(gpbdev_tree_t* out, int device, int64_t n, int F, 
   TCUDA(cudaSetDevice(device));
   gpbdev_tree* h = new gpbdev_tree();
   h->device = device; h->n = n; h->F = F; h->Fpad = (F + 31) / 32 * 32; h->L = cfg->num_leaves; h->cfg = *cfg;
+  // With both limits at 0 a threshold past a leaf's last occupied bin is admissible and gains (sum g)^2 (1/(H + eps) - 1/(H + 2 eps))
+  // > 0 when the hessian sum H is small: a split with an empty child, which the partition cannot produce. The reference raises
+  // min_data_in_leaf to 1 in that case (Config::CheckParamConflict, io/config.cpp:400-405).
+  if (h->cfg.min_data_in_leaf <= 0 && h->cfg.min_sum_hessian_in_leaf <= kEps) h->cfg.min_data_in_leaf = 1;
   cudaDeviceProp prop;
   TCUDA(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;

@@ -37,7 +37,8 @@ def P(a, t):
     return a.ctypes.data_as(C.POINTER(t))
 
 
-def dev_train(lib, bins_fm, num_bin, grad, cfg):
+def dev_train(lib, bins_fm, num_bin, grad, cfg, on_device=False):
+    """on_device: the gradient goes through a device buffer (the only way into the graph-replayed leaf loop)"""
     F, n = bins_fm.shape
     h = C.c_void_p()
     dc = DevCfg(cfg.num_leaves, cfg.min_data_in_leaf, cfg.min_sum_hessian_in_leaf, cfg.lambda_l2, cfg.min_gain_to_split, cfg.max_depth)
@@ -49,8 +50,15 @@ def dev_train(lib, bins_fm, num_bin, grad, cfg):
     sf = np.zeros(L, np.int32); tb = np.zeros(L, np.int32); lc = np.zeros(L, np.int32); rcd = np.zeros(L, np.int32)
     sg = np.zeros(L, np.float32); lv = np.zeros(L, np.float64); cnt = np.zeros(L, np.int32)
     g = np.ascontiguousarray(grad, dtype=np.float64)
-    rc = lib.gpbdev_tree_train(h, P(g, C.c_double), 0, C.c_double(1.0), C.byref(nl), P(sf, C.c_int), P(tb, C.c_int), P(lc, C.c_int), P(rcd, C.c_int),
+    gp = P(g, C.c_double)
+    if on_device:
+        gp = C.c_void_p()
+        assert lib.gpbdev_vec_alloc(h, C.byref(gp), C.c_int64(n)) == 0
+        assert lib.gpbdev_vec_upload(h, gp, P(g, C.c_double), C.c_int64(n)) == 0
+    rc = lib.gpbdev_tree_train(h, gp, 1 if on_device else 0, C.c_double(1.0), C.byref(nl), P(sf, C.c_int), P(tb, C.c_int), P(lc, C.c_int), P(rcd, C.c_int),
                                P(sg, C.c_float), P(lv, C.c_double), P(cnt, C.c_int))
+    if on_device:
+        lib.gpbdev_vec_free(h, gp)
     assert rc == 0, lib.gpbdev_tree_last_error().decode()
     k = nl.value
     lib.gpbdev_tree_free(h)
@@ -87,7 +95,8 @@ VARIANTS = {
 @pytest.mark.parametrize("variant", list(VARIANTS))
 def test_tree_kernel_variants_match_oracle(lib, tree_golden, variant, monkeypatch):
     """Same parity bar for every kernel variant: oracle trees (incl. binary and constant-heavy features, F > 64, a leaf budget
-    the data cannot fill) through gpbdev_tree_train, and one reference golden through the Booster (device-resident gradients)."""
+    the data cannot fill) through gpbdev_tree_train (host gradients, device-resident ones for the graph loop), and one reference
+    golden through the Booster (device-resident gradients). tests/test_tree_kernels_gpu.py covers every kernel combination."""
     for k, v in VARIANTS[variant].items():
         monkeypatch.setenv(k, v)
     for n, F, levels, L, mdl in [(30000, 40, 255, 31, 20), (10000, 70, 16, 63, 3), (500, 3, 5, 31, 1), (20000, 9, 2, 16, 50), (50, 2, 4, 4, 30)]:
@@ -96,7 +105,7 @@ def test_tree_kernel_variants_match_oracle(lib, tree_golden, variant, monkeypatc
         grad = rng.standard_normal(n) + (bins[0] > levels // 2) * 0.8 - (bins[min(1, F - 1)] % 3 == 0) * 0.5
         cfg = ot.make_config(num_leaves=L, min_data_in_leaf=mdl)
         a = ot.train_tree(bins, np.full(F, levels), grad, cfg)
-        d = dev_train(lib, bins, np.full(F, levels), grad, cfg)
+        d = dev_train(lib, bins, np.full(F, levels), grad, cfg, on_device=variant == "graph_loop")
         assert d["num_leaves"] == a["num_leaves"], (variant, n, F)
         for k in ("split_feature", "threshold_bin", "left_child", "right_child", "leaf_count"):
             assert np.array_equal(d[k], a[k]), (variant, n, F, k)
