@@ -395,6 +395,7 @@ struct gpbdev_dense {
   double* out_host = nullptr;
   int64_t launches = 0;
   bool factored = false;
+  bool psi_inv_ready = false;  // P holds Psi^-1 of the current factor
 };
 
 extern "C" {
@@ -423,8 +424,11 @@ int gpbdev_dense_create(gpbdev_dense_t* out, int device, int n, int d, const dou
   DCUDA(cudaMalloc(&h->out, sizeof(double) * 4));
   DCUDA(cudaMalloc(&h->info, sizeof(int)));
   DCUDA(cudaMallocHost(&h->out_host, sizeof(double) * 4));
-  DCUDA(cudaMemcpy(h->coords, coords_rowmajor, sizeof(double) * (size_t)n * d, cudaMemcpyHostToDevice));
-  DCUDA(cudaMemset(h->y, 0, sizeof(double) * n));
+  // on the engine's stream: it does not wait for the legacy default stream, so a cudaMemset there could land after the
+  // first set_y and zero the response
+  DCUDA(cudaMemcpyAsync(h->coords, coords_rowmajor, sizeof(double) * (size_t)n * d, cudaMemcpyHostToDevice, h->stream));
+  DCUDA(cudaMemsetAsync(h->y, 0, sizeof(double) * n, h->stream));
+  DCUDA(cudaStreamSynchronize(h->stream));
   DCUDA(cudaFuncSetAttribute(syrk_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 2 * NB * (NB + 1))));
   *out = h;
   return 0;
@@ -447,6 +451,7 @@ int gpbdev_dense_set_y(gpbdev_dense_t h, const double* y_host) {
   DCUDA(cudaMemcpyAsync(h->y, y_host, sizeof(double) * h->n, cudaMemcpyHostToDevice, h->stream));
   DCUDA(cudaStreamSynchronize(h->stream));
   h->factored = false;
+  h->psi_inv_ready = false;
   return 0;
 }
 
@@ -456,6 +461,7 @@ int gpbdev_dense_eval(gpbdev_dense_t h, int cov_type, double var, double range, 
   if (!(var > 0.) || !(range > 0.)) return dfail("gpbdev_dense_eval: covariance parameters must be positive");
   DCUDA(cudaSetDevice(h->device));
   const int n = h->n, nt = h->nt, ld = h->ld;
+  h->psi_inv_ready = false;
   DCUDA(cudaMemsetAsync(h->info, 0, sizeof(int), h->stream));
   pick_gram(cov_type)<<<dim3(nt, nt), 256, 0, h->stream>>>(h->coords, n, h->d, h->y, var, range, h->A, ld);
   DCUDA(cudaGetLastError());
@@ -524,6 +530,7 @@ int gpbdev_dense_grad(gpbdev_dense_t h, double* out4) {
   out4[2] = quad - aa;          // alpha^T (Psi - I) alpha = alpha^T y - alpha^T alpha
   out4[3] = s_aga;
   h->out_host[0] = quad;
+  h->psi_inv_ready = true;
   return 0;
 }
 
@@ -536,6 +543,39 @@ int gpbdev_dense_yaux(gpbdev_dense_t h, double scale, double* yaux_host) {
   h->launches += 1;
   DCUDA(cudaMemcpyAsync(yaux_host, h->x, sizeof(double) * h->n, cudaMemcpyDeviceToHost, h->stream));
   DCUDA(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// Read-back of the factor for tests. Only the lower triangle of the diagonal tiles is the factor (the trailing update
+// writes whole diagonal tiles, and tiles above the diagonal are never written), so the upper triangle is zeroed here.
+int gpbdev_dense_get_factor(gpbdev_dense_t h, double* L_host, double* z_host) {
+  if (!h || !L_host) return dfail("gpbdev_dense_get_factor: null argument");
+  if (!h->factored) return dfail("gpbdev_dense_get_factor: no current factor (call gpbdev_dense_eval after gpbdev_dense_set_y)");
+  DCUDA(cudaSetDevice(h->device));
+  const size_t n = (size_t)h->n, ld = (size_t)h->ld;
+  DCUDA(cudaMemcpy2DAsync(L_host, sizeof(double) * n, h->A, sizeof(double) * ld, sizeof(double) * n, n, cudaMemcpyDeviceToHost,
+                          h->stream));
+  if (z_host) DCUDA(cudaMemcpyAsync(z_host, h->A + n * ld, sizeof(double) * n, cudaMemcpyDeviceToHost, h->stream));
+  DCUDA(cudaStreamSynchronize(h->stream));
+  for (size_t r = 0; r < n; ++r) std::fill(L_host + r * n + r + 1, L_host + (r + 1) * n, 0.);
+  return 0;
+}
+
+// Read-back of Psi^-1 for tests: block row I of P is copied up to its diagonal tile (the upper tiles are never written),
+// then the strict lower triangle is mirrored.
+int gpbdev_dense_get_psi_inv(gpbdev_dense_t h, double* P_host) {
+  if (!h || !P_host) return dfail("gpbdev_dense_get_psi_inv: null argument");
+  if (!h->factored || !h->psi_inv_ready) return dfail("gpbdev_dense_get_psi_inv: no current Psi^-1 (call gpbdev_dense_grad after gpbdev_dense_eval)");
+  DCUDA(cudaSetDevice(h->device));
+  const size_t n = (size_t)h->n, ld = (size_t)h->ld;
+  for (size_t r0 = 0; r0 < n; r0 += NB) {
+    const size_t rows = std::min<size_t>(NB, n - r0), cols = std::min(r0 + NB, n);
+    DCUDA(cudaMemcpy2DAsync(P_host + r0 * n, sizeof(double) * n, h->P + r0 * ld, sizeof(double) * ld, sizeof(double) * cols, rows,
+                            cudaMemcpyDeviceToHost, h->stream));
+  }
+  DCUDA(cudaStreamSynchronize(h->stream));
+  for (size_t r = 0; r < n; ++r)
+    for (size_t c = r + 1; c < n; ++c) P_host[r * n + c] = P_host[c * n + r];
   return 0;
 }
 

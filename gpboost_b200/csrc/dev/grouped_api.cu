@@ -103,6 +103,7 @@ struct gpbdev_grouped {
   double* out_host = nullptr;
   double* stage = nullptr;
   int64_t launches = 0;
+  bool has_y = false;  // s / yy hold the sums of an installed response
 };
 
 extern "C" {
@@ -112,6 +113,15 @@ const char* gpbdev_grouped_last_error(void) { return g_grp_err.c_str(); }
 int gpbdev_grouped_create(gpbdev_grouped_t* out, int device, int64_t n, const int32_t* group_index, int num_groups) {
   if (!out || !group_index) return gfail("gpbdev_grouped_create: null argument");
   if (n <= 0 || num_groups <= 0) return gfail("gpbdev_grouped_create: need n > 0 and at least one group");
+  // the host-side grouping is validated before any device resource exists
+  std::vector<int32_t> offs(num_groups + 1, 0), perm(n);
+  for (int64_t i = 0; i < n; ++i) {
+    if (group_index[i] < 0 || group_index[i] >= num_groups) return gfail("gpbdev_grouped_create: group index out of range");
+    ++offs[group_index[i] + 1];
+  }
+  for (int g = 0; g < num_groups; ++g) offs[g + 1] += offs[g];
+  std::vector<int32_t> fill(offs.begin(), offs.end() - 1);
+  for (int64_t i = 0; i < n; ++i) perm[fill[group_index[i]]++] = (int32_t)i;  // stable: ascending i inside a group
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= device) {
     cudaGetLastError();
@@ -124,14 +134,6 @@ int gpbdev_grouped_create(gpbdev_grouped_t* out, int device, int64_t n, const in
   GCUDA(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;
   GCUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  std::vector<int32_t> offs(num_groups + 1, 0), perm(n);
-  for (int64_t i = 0; i < n; ++i) {
-    if (group_index[i] < 0 || group_index[i] >= num_groups) { delete h; return gfail("gpbdev_grouped_create: group index out of range"); }
-    ++offs[group_index[i] + 1];
-  }
-  for (int g = 0; g < num_groups; ++g) offs[g + 1] += offs[g];
-  std::vector<int32_t> fill(offs.begin(), offs.end() - 1);
-  for (int64_t i = 0; i < n; ++i) perm[fill[group_index[i]]++] = (int32_t)i;  // stable: ascending i inside a group
   GCUDA(cudaMalloc(&h->perm, sizeof(int32_t) * n));
   GCUDA(cudaMalloc(&h->offs, sizeof(int32_t) * (num_groups + 1)));
   GCUDA(cudaMalloc(&h->y, sizeof(double) * n));
@@ -141,8 +143,10 @@ int gpbdev_grouped_create(gpbdev_grouped_t* out, int device, int64_t n, const in
   GCUDA(cudaMalloc(&h->out, sizeof(double) * 8));
   GCUDA(cudaMallocHost(&h->out_host, sizeof(double) * 8));
   GCUDA(cudaMallocHost(&h->stage, sizeof(double) * n));
-  GCUDA(cudaMemcpy(h->perm, perm.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice));
-  GCUDA(cudaMemcpy(h->offs, offs.data(), sizeof(int32_t) * (num_groups + 1), cudaMemcpyHostToDevice));
+  // on the engine's stream (it does not wait for the legacy default stream), complete before the first set_y
+  GCUDA(cudaMemcpyAsync(h->perm, perm.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, h->stream));
+  GCUDA(cudaMemcpyAsync(h->offs, offs.data(), sizeof(int32_t) * (num_groups + 1), cudaMemcpyHostToDevice, h->stream));
+  GCUDA(cudaStreamSynchronize(h->stream));
   *out = h;
   return 0;
 }
@@ -166,6 +170,7 @@ int gpbdev_grouped_set_y(gpbdev_grouped_t h, const double* y_host) {
   group_sums_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->y, h->perm, h->offs, h->G, h->s, h->yy);
   GCUDA(cudaGetLastError());
   h->launches += 1;
+  h->has_y = true;
   return 0;
 }
 
@@ -176,12 +181,14 @@ int gpbdev_grouped_set_y_device(gpbdev_grouped_t h, const double* y_dev) {
   group_sums_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->y, h->perm, h->offs, h->G, h->s, h->yy);
   GCUDA(cudaGetLastError());
   h->launches += 1;
+  h->has_y = true;
   return 0;
 }
 
 int gpbdev_grouped_eval(gpbdev_grouped_t h, double var_ratio, double* out5) {
   if (!h || !out5) return gfail("gpbdev_grouped_eval: null argument");
   if (!(var_ratio > 0.)) return gfail("gpbdev_grouped_eval: the variance ratio must be positive");
+  if (!h->has_y) return gfail("gpbdev_grouped_eval: no response installed (call gpbdev_grouped_set_y first)");
   GCUDA(cudaSetDevice(h->device));
   group_eval_kernel<<<1, 256, 0, h->stream>>>(h->s, h->yy, h->offs, h->G, var_ratio, h->out);
   GCUDA(cudaGetLastError());
@@ -194,6 +201,7 @@ int gpbdev_grouped_eval(gpbdev_grouped_t h, double var_ratio, double* out5) {
 
 int gpbdev_grouped_yaux(gpbdev_grouped_t h, double var_ratio, double scale, double* yaux_host) {
   if (!h || !yaux_host) return gfail("gpbdev_grouped_yaux: null argument");
+  if (!h->has_y) return gfail("gpbdev_grouped_yaux: no response installed (call gpbdev_grouped_set_y first)");
   GCUDA(cudaSetDevice(h->device));
   group_yaux_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->y, h->perm, h->offs, h->s, h->G, var_ratio, scale, h->yaux);
   GCUDA(cudaGetLastError());
@@ -206,6 +214,7 @@ int gpbdev_grouped_yaux(gpbdev_grouped_t h, double var_ratio, double scale, doub
 
 int gpbdev_grouped_yaux_device(gpbdev_grouped_t h, double var_ratio, double scale, double* out_dev) {
   if (!h || !out_dev) return gfail("gpbdev_grouped_yaux_device: null argument");
+  if (!h->has_y) return gfail("gpbdev_grouped_yaux_device: no response installed (call gpbdev_grouped_set_y first)");
   GCUDA(cudaSetDevice(h->device));
   group_yaux_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->y, h->perm, h->offs, h->s, h->G, var_ratio, scale, out_dev);
   GCUDA(cudaGetLastError());

@@ -169,6 +169,11 @@ GPBDEV_EXPORT int gpbdev_dense_yaux(gpbdev_dense_t h, double scale, double* yaux
 /* gradient sums at the parameters of the last gpbdev_dense_eval (CalcPsiInv re_model_template.h:6586-6617 + the dense branch of
  * CalcGradPars :2018-2039): out4 = {tr(Psi^-1 Sigma), tr(Psi^-1 dSigma/dlog range), alpha^T Sigma alpha, alpha^T dSigma/dlog range alpha} */
 GPBDEV_EXPORT int gpbdev_dense_grad(gpbdev_dense_t h, double* out4);
+/* After gpbdev_dense_eval (and no set_y since): L_host (n x n row-major) = the Cholesky factor of Psi, zeros above the diagonal;
+ * z_host (n, may be NULL) = L^-1 y, the response row of the factored matrix. Read-back for tests. */
+GPBDEV_EXPORT int gpbdev_dense_get_factor(gpbdev_dense_t h, double* L_host, double* z_host);
+/* After gpbdev_dense_grad (and no eval or set_y since): P_host (n x n row-major) = Psi^-1, both triangles. Read-back for tests. */
+GPBDEV_EXPORT int gpbdev_dense_get_psi_inv(gpbdev_dense_t h, double* P_host);
 GPBDEV_EXPORT int64_t gpbdev_dense_launch_count(gpbdev_dense_t h);
 
 /* ------------------------------------------------------------------------------------------------------------------
@@ -183,7 +188,7 @@ GPBDEV_EXPORT int gpbdev_grouped_free(gpbdev_grouped_t h);
 /* y in original order (host): H2D + per-group sums Z^T y (SetY / CalcZtY) */
 GPBDEV_EXPORT int gpbdev_grouped_set_y(gpbdev_grouped_t h, const double* y_host);
 /* sums at variance ratio v = sigma_1^2/sigma^2: out5 = { y'y, sum s_g^2/(1/v+n_g), sum log(1+v n_g),
- * sum s_g^2 v/(1+v n_g)^2, sum v n_g/(1+v n_g) } */
+ * sum s_g^2 v/(1+v n_g)^2, sum v n_g/(1+v n_g) }. This and the yaux entries fail until a response is installed. */
 GPBDEV_EXPORT int gpbdev_grouped_eval(gpbdev_grouped_t h, double var_ratio, double* out5);
 /* y_aux = Psi^-1 y * scale in original order (CalcYAux single-RE branch) */
 GPBDEV_EXPORT int gpbdev_grouped_yaux(gpbdev_grouped_t h, double var_ratio, double scale, double* yaux_host);
