@@ -394,6 +394,22 @@ int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, i
                 "] for the CUDA Vecchia engine");
   if ((int64_t)n * m >= (int64_t)2147483647) return fail("gpbdev_vecchia_create: n * num_neighbors exceeds int32 positions");
   if (row_begin < 0 || row_end > n || row_begin > row_end) return fail("gpbdev_vecchia_create: bad row shard");
+  if (nn) {
+    // Supplied neighbour sets. The Laplace triangular solves poll the rows a row depends on until they are written, which only
+    // ends if every dependency comes earlier in the order: each entry must be -1 (padding) or an earlier row, at most once per row.
+    std::vector<int64_t> seen((size_t)n, -1);
+    for (int64_t i = 0; i < n; ++i)
+      for (int k = 0; k < m; ++k) {
+        const int32_t j = nn[i * m + k];
+        if (j == -1) continue;
+        if (j < -1 || j >= i)
+          return fail("gpbdev_vecchia_create: neighbour " + std::to_string(j) + " of row " + std::to_string(i) +
+                      " is neither -1 nor an earlier row");
+        if (seen[(size_t)j] == i)
+          return fail("gpbdev_vecchia_create: neighbour " + std::to_string(j) + " appears twice in row " + std::to_string(i));
+        seen[(size_t)j] = i;
+      }
+  }
   if (gpbdev_device_count() <= device)
     return fail("gpbdev_vecchia_create: no CUDA device " + std::to_string(device) + " — the CUDA engine has no CPU fallback");
   CUDA_TRY(cudaSetDevice(device));

@@ -1212,6 +1212,39 @@ int lap_check_err(gpbdev_vecchia* h) {
   return 0;
 }
 
+// one operator of gpbdev_vecchia_laplace_apply on device multi-vectors X, X2 (n x t); out receives the result, scr is scratch
+int lap_apply_run(gpbdev_vecchia* h, int op, int t, const double* X, const double* X2, double* out, double* scr, double* dots) {
+  gpb_laplace_state* L = h->lap;
+  const int64_t n = h->n;
+  const int G = lap_groups(t), grid = lap_grid(L->grid_mv, G);
+  double scratch_dots[gpl::kMaxCols];
+  CUDA_TRY(cudaMemsetAsync(L->err, 0, sizeof(int), h->stream));
+  switch (op) {
+    case 0: if (lap_mv_B(h, t, h->Dinv, X, out)) return -1; break;
+    case 1: {
+      int prow = 0;
+      if (lap_mv_Bt(h, t, X, L->W, X2, out, &prow)) return -1;
+      if (laplace_colsums(h, t, dots, prow)) return -1;
+      break;
+    }
+    case 2: if (lap_apply_op(h, t, X, out, scr, dots)) return -1; break;
+    case 3: if (lap_precond(h, t, X, out, scr, dots)) return -1; break;
+    case 4: if (lap_precond(h, t, X, scr, out, scratch_dots)) return -1; break;  // out = the Y buffer: B^-T X
+    case 5:
+      gpl::mv_Bg_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->dA, h->nn, h->m, n, t, G, X, out);
+      CUDA_TRY(cudaGetLastError());
+      h->launches += 1;
+      break;
+    default:
+      CUDA_TRY(cudaMemcpyAsync(out, X2, sizeof(double) * (size_t)n * t, cudaMemcpyDeviceToDevice, h->stream));
+      gpl::mv_Bgt_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->dA, h->colptr, h->csc_pos, h->m, n, t, G, X, out, 1);
+      CUDA_TRY(cudaGetLastError());
+      h->launches += 1;
+      break;
+  }
+  return lap_check_err(h);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1651,6 +1684,53 @@ int gpbdev_vecchia_laplace_get_mode(gpbdev_vecchia_t h, double* mode_host) {
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   std::memcpy(mode_host, L->stage, sizeof(double) * h->n);
   return 0;
+}
+
+// Test read-back of one operator (include/gpboost_b200_dev.h). Leaves W, dw and the factor as an evaluation would overwrite them
+// anyway; the kept SLQ solutions are invalidated, so a gradient needs a new evaluation first.
+int gpbdev_vecchia_laplace_apply(gpbdev_vecchia_t h, int cov_type, double var, double range, int op, int t, const double* W_host,
+                                 const double* X_host, const double* X2_host, double* out_host, double* dots_host) {
+  if (!h) return fail("gpbdev_vecchia_laplace_apply: null handle");
+  if (op < 0 || op > 6) return fail("gpbdev_vecchia_laplace_apply: unknown operator " + std::to_string(op));
+  if (t < 1 || t > gpl::kMaxCols) return fail("gpbdev_vecchia_laplace_apply: t must be in [1, 128]");
+  if (h->m > gpl::kM) return fail("gpbdev_vecchia_laplace_apply: num_neighbors must be <= 30");
+  const bool need_x2 = op == 1 || op == 6, need_dots = op >= 1 && op <= 3;
+  if (!W_host || !X_host || !out_host || (need_x2 && !X2_host) || (need_dots && !dots_host))
+    return fail("gpbdev_vecchia_laplace_apply: null buffer");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (laplace_ensure(h)) return -1;
+  gpb_laplace_state* L = h->lap;
+  L->solutions_valid = false;
+  if (launch_eval(h, cov_type, var, range, gpb::MODE_STORE_GRAD, true)) return -1;
+  if (ensure_csc(h)) return -1;
+  if (lap_refresh_csc_coefs(h)) return -1;
+  const int64_t n = h->n;
+  std::vector<double> dw((size_t)n);
+  CUDA_TRY(cudaMemcpyAsync(dw.data(), h->Dinv, sizeof(double) * n, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  for (int64_t i = 0; i < n; ++i) dw[(size_t)i] += W_host[i];
+  CUDA_TRY(cudaMemcpyAsync(L->W, W_host, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(L->dw, dw.data(), sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+  const size_t bytes = sizeof(double) * (size_t)n * t;
+  double *X = nullptr, *X2 = nullptr, *out = nullptr, *scr = nullptr;
+  cudaError_t e = cudaMalloc(&X, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&X2, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&out, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&scr, bytes);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(X, X_host, bytes, cudaMemcpyHostToDevice, h->stream);
+  if (e == cudaSuccess && need_x2) e = cudaMemcpyAsync(X2, X2_host, bytes, cudaMemcpyHostToDevice, h->stream);
+  int rc = e == cudaSuccess ? 0 : fail(std::string("gpbdev_vecchia_laplace_apply: ") + cudaGetErrorString(e));
+  double dots[gpl::kMaxCols];
+  if (rc == 0) rc = lap_apply_run(h, op, t, X, X2, out, scr, dots);
+  if (rc == 0) {
+    e = cudaMemcpyAsync(out_host, out, bytes, cudaMemcpyDeviceToHost, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) rc = fail(std::string("gpbdev_vecchia_laplace_apply: ") + cudaGetErrorString(e));
+    else if (need_dots) std::memcpy(dots_host, dots, sizeof(double) * t);
+  }
+  cudaStreamSynchronize(h->stream);
+  cudaFree(X); cudaFree(X2); cudaFree(out); cudaFree(scr);
+  return rc;
 }
 
 }  // extern "C"

@@ -220,7 +220,8 @@ vecchia_factor_kernel(const FactorArgs p) {
 #pragma unroll
       for (int k = 0; k < (DIM > 0 ? DIM : 1); ++k) my[k] = pts[lane * dim + k];
     }
-    const bool full = (q == MT);  // warp-uniform: no dummy slots (every row i >= m of a model with m == MT)
+    // warp-uniform: no dummy slots (rows i >= m of a model with m == MT, unless supplied neighbour sets pad them with -1)
+    const bool full = real_mask == (1u << P) - 1u;
 #pragma unroll
     for (int t = 1; t <= NT; ++t) {
       int o = lane + t;

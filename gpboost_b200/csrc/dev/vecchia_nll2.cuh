@@ -182,7 +182,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MODE == MODE_GRAD ? GPB_N
     // which point slots of my half are real (bit s): slots 0..q-1 and slot MT
     const unsigned blo = __ballot_sync(0xffffffffu, real_lo), bhi = __ballot_sync(0xffffffffu, real_hi);
     const unsigned real_mask = ((blo >> hbase) & 0xffffu) | (((bhi >> hbase) & 0xffffu) << 16);
-    const bool full = (__all_sync(0xffffffffu, (q == MT) || !active)) != 0;  // no dummy slots anywhere in the warp
+    // no dummy slots anywhere in the warp (supplied neighbour sets may pad rows i >= m with -1 too)
+    const bool full = (__all_sync(0xffffffffu, real_mask == (1u << P) - 1u || !active)) != 0;
     const bool was_active = active;
     // next pair
     const int64_t it_n = it + nwarps;

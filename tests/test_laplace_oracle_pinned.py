@@ -149,7 +149,8 @@ def test_device_gradient_schedule_matches_reference(idx):
     """The operator schedule of gpbdev_vecchia_laplace_grad (csrc/dev/laplace.cuh) replayed in numpy — the same sequence of
     products with B, B^T, B_grad, B_grad^T, the same coefficient vectors c1 = -D^-1 dD, c2 = D^-1 + W, c3 = 1 + W / D^-1, the same
     buffers and signs — on the oracle's factor, mode, probes and CG solutions: it must give the reference's gradient. (The kernels
-    themselves are checked on the GPU; this pins the algebra they are composed with.)"""
+    themselves are checked one by one against a longdouble reference in tests/test_laplace_kernels_gpu.py; this pins the algebra
+    they are composed with.)"""
     import scipy.sparse as sp
     c = GOLD[idx]
     X, y, off = data_of(c)
