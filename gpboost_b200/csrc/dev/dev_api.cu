@@ -444,34 +444,13 @@ int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, i
     CUDA_TRY(cudaMemcpy(h->nn, nn, sizeof(int32_t) * n * m, cudaMemcpyHostToDevice));
     h->nn_host.assign(nn, nn + (size_t)n * m);
   } else {
-    // rank of every point in the sorted coordinate sums (Vecchia_utils.cpp:775-786). The permutation of
-    // equal sums is whatever std::sort yields, so the same library call is made on the same input.
-    std::vector<double> csum((size_t)n);
-    for (int64_t i = 0; i < n; ++i) {
-      double sacc = 0.;
-      for (int k = 0; k < d; ++k) sacc += coords_ordered[i * d + k];
-      csum[(size_t)i] = sacc;
-    }
-    std::vector<int> sort_sum((size_t)n);
-    std::iota(sort_sum.begin(), sort_sum.end(), 0);
-    std::sort(sort_sum.begin(), sort_sum.end(), [&csum](int i1, int i2) { return csum[i1] < csum[i2]; });
-    std::vector<int32_t> pos((size_t)n);
-    for (int64_t r = 0; r < n; ++r) pos[(size_t)sort_sum[(size_t)r]] = (int32_t)r;
-    int32_t *pos_dev = nullptr, *sort_sum_dev = nullptr;
-    double* csum_dev = nullptr;
-    CUDA_TRY(cudaMalloc(&pos_dev, sizeof(int32_t) * n));
-    CUDA_TRY(cudaMalloc(&sort_sum_dev, sizeof(int32_t) * n));
-    CUDA_TRY(cudaMalloc(&csum_dev, sizeof(double) * n));
-    CUDA_TRY(cudaMemcpy(pos_dev, pos.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(sort_sum_dev, sort_sum.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(csum_dev, csum.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
     std::string err;
-    const int nl = gpb::knn_vecchia_device(h->coords, coords_ordered, n, d, m, pos_dev, sort_sum_dev, csum_dev, h->nn, h->stream,
-                                           h->num_sms, &h->knn_replayed, &err);
-    cudaFree(pos_dev); cudaFree(sort_sum_dev); cudaFree(csum_dev);
+    gpb::KnnInfo info;
+    const int nl = gpb::knn_vecchia_search(h->coords, coords_ordered, n, d, m, h->nn, h->stream, h->num_sms, &info, &err,
+                                           /*q_begin=*/0, /*end_search_at=*/n - 2);
     if (nl < 0) { gpbdev_vecchia_free(h); return fail("gpbdev_vecchia_create: device neighbour search failed: " + err); }
     h->launches += nl;
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
+    h->knn_replayed = (int)info.replayed;
   }
   *out = h;
   return 0;
@@ -627,35 +606,18 @@ int gpbdev_vecchia_predict(gpbdev_vecchia_t h, int cov_type, double var, double 
   std::vector<double> call((size_t)na * d);
   CUDA_TRY(cudaMemcpy(call.data(), h->coords, sizeof(double) * n * d, cudaMemcpyDeviceToHost));
   std::memcpy(call.data() + (size_t)n * d, coords_pred_host, sizeof(double) * np * d);
-  std::vector<double> csum((size_t)na);
-  for (int64_t i = 0; i < na; ++i) {
-    double sacc = 0.;
-    for (int k = 0; k < d; ++k) sacc += call[(size_t)i * d + k];
-    csum[(size_t)i] = sacc;
-  }
-  std::vector<int> sort_sum((size_t)na);
-  std::iota(sort_sum.begin(), sort_sum.end(), 0);
-  std::sort(sort_sum.begin(), sort_sum.end(), [&csum](int i1, int i2) { return csum[i1] < csum[i2]; });
-  std::vector<int32_t> pos((size_t)na);
-  for (int64_t r = 0; r < na; ++r) pos[(size_t)sort_sum[(size_t)r]] = (int32_t)r;
-  double *call_dev = nullptr, *csum_dev = nullptr, *mean_dev = nullptr, *var_dev = nullptr;
-  int32_t *pos_dev = nullptr, *sort_dev = nullptr, *nnp = nullptr;
-  auto release = [&]() { cudaFree(call_dev); cudaFree(csum_dev); cudaFree(mean_dev); cudaFree(var_dev); cudaFree(pos_dev); cudaFree(sort_dev); cudaFree(nnp); };
+  double *call_dev = nullptr, *mean_dev = nullptr, *var_dev = nullptr;
+  int32_t* nnp = nullptr;
+  auto release = [&]() { cudaFree(call_dev); cudaFree(mean_dev); cudaFree(var_dev); cudaFree(nnp); };
   cudaError_t e = cudaMalloc(&call_dev, sizeof(double) * na * d);
-  if (e == cudaSuccess) e = cudaMalloc(&csum_dev, sizeof(double) * na);
-  if (e == cudaSuccess) e = cudaMalloc(&pos_dev, sizeof(int32_t) * na);
-  if (e == cudaSuccess) e = cudaMalloc(&sort_dev, sizeof(int32_t) * na);
   if (e == cudaSuccess) e = cudaMalloc(&nnp, sizeof(int32_t) * np * mp);
   if (e == cudaSuccess) e = cudaMalloc(&mean_dev, sizeof(double) * np);
   if (e == cudaSuccess) e = cudaMalloc(&var_dev, sizeof(double) * np);
   if (e == cudaSuccess) e = cudaMemcpy(call_dev, call.data(), sizeof(double) * na * d, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(csum_dev, csum.data(), sizeof(double) * na, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(pos_dev, pos.data(), sizeof(int32_t) * na, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(sort_dev, sort_sum.data(), sizeof(int32_t) * na, cudaMemcpyHostToDevice);
   if (e != cudaSuccess) { release(); return fail(std::string("gpbdev_vecchia_predict: ") + cudaGetErrorString(e)); }
   std::string err;
-  int replayed = 0;
-  const int nl = gpb::knn_vecchia_device(call_dev, call.data(), na, d, mp, pos_dev, sort_dev, csum_dev, nnp, h->stream, h->num_sms, &replayed, &err,
+  gpb::KnnInfo info;
+  const int nl = gpb::knn_vecchia_search(call_dev, call.data(), na, d, mp, nnp, h->stream, h->num_sms, &info, &err,
                                          /*q_begin=*/n, /*end_search_at=*/n - 1);
   if (nl < 0) { release(); return fail("gpbdev_vecchia_predict: device neighbour search failed: " + err); }
   h->launches += nl;
@@ -725,6 +687,48 @@ int gpbdev_vecchia_sync(gpbdev_vecchia_t h) {
 }
 int64_t gpbdev_vecchia_launch_count(gpbdev_vecchia_t h) { return h ? h->launches : 0; }
 int gpbdev_vecchia_knn_replayed(gpbdev_vecchia_t h) { return h ? h->knn_replayed : 0; }
+
+int gpbdev_knn_search(int device, const double* coords_host, int64_t n, int d, int m, int64_t q_begin, int64_t end_search_at,
+                      int32_t* nn_host, int64_t* info_out) {
+  if (!coords_host || !nn_host || !info_out) return fail("gpbdev_knn_search: null argument");
+  if (d < 1) return fail("gpbdev_knn_search: need dim >= 1");
+  if (m < 1 || m > gpb::kBigMaxNeighbors)
+    return fail("gpbdev_knn_search: num_neighbors must be in [1, " + std::to_string(gpb::kBigMaxNeighbors) + "]");
+  if (n < 1 || n >= (int64_t)2147483647) return fail("gpbdev_knn_search: need 1 <= n < 2^31");
+  if (q_begin < 0 || q_begin >= n) return fail("gpbdev_knn_search: q_begin must be in [0, n)");
+  if (end_search_at != (q_begin == 0 ? n - 2 : q_begin - 1))
+    return fail("gpbdev_knn_search: end_search_at must be n - 2 for model queries (q_begin = 0) and q_begin - 1 for prediction");
+  m = (int)std::min<int64_t>(m, end_search_at + 1);  // Vecchia_utils.cpp:752-755
+  if (m < 1) return fail("gpbdev_knn_search: model queries need n >= 2");
+  const int64_t nq = n - q_begin;
+  if (nq * m >= (int64_t)2147483647) return fail("gpbdev_knn_search: n * num_neighbors exceeds int32 positions");
+  if (gpbdev_device_count() <= device) return fail("gpbdev_knn_search: no CUDA device " + std::to_string(device));
+  CUDA_TRY(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+  cudaStream_t stream = nullptr;
+  double* coords_dev = nullptr;
+  int32_t* nn_dev = nullptr;
+  CUDA_TRY(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+  auto release = [&]() { cudaFree(coords_dev); cudaFree(nn_dev); cudaStreamDestroy(stream); };
+  cudaError_t e = cudaMalloc(&coords_dev, sizeof(double) * n * d);
+  if (e == cudaSuccess) e = cudaMalloc(&nn_dev, sizeof(int32_t) * nq * m);
+  if (e == cudaSuccess) e = cudaMemcpy(coords_dev, coords_host, sizeof(double) * n * d, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) { release(); return fail(std::string("gpbdev_knn_search: ") + cudaGetErrorString(e)); }
+  std::string err;
+  gpb::KnnInfo info;
+  if (gpb::knn_vecchia_search(coords_dev, coords_host, n, d, m, nn_dev, stream, prop.multiProcessorCount, &info, &err, q_begin,
+                              end_search_at) < 0) {
+    release();
+    return fail("gpbdev_knn_search: " + err);
+  }
+  e = cudaMemcpy(nn_host, nn_dev, sizeof(int32_t) * nq * m, cudaMemcpyDeviceToHost);
+  release();
+  if (e != cudaSuccess) return fail(std::string("gpbdev_knn_search: ") + cudaGetErrorString(e));
+  const int64_t vals[7] = {info.replayed, info.launches, info.brute_end, info.ncell, info.g[0], info.g[1], info.g[2]};
+  std::memcpy(info_out, vals, sizeof(vals));
+  return 0;
+}
 
 int gpbdev_fp64_peak(int device, double* tflops) {
   if (!tflops) return fail("null argument");

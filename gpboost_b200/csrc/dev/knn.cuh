@@ -24,7 +24,9 @@
 #include <algorithm>
 #include <cmath>
 #include <cub/device/device_radix_sort.cuh>
+#include <numeric>
 #include <string>
+#include <vector>
 
 namespace gpb {
 
@@ -34,6 +36,16 @@ struct KnnGrid {
   double hmin;
   int g[3];
   int dim;
+};
+
+// What one search did (test read-back gpbdev_knn_search): queries re-derived by the exact replay, kernels launched, first query
+// of the cell-list search (= n when every query is brute force) and the cell grid (ncell = 0, g = 0 without one).
+struct KnnInfo {
+  int64_t replayed = 0;
+  int64_t launches = 0;
+  int64_t brute_end = 0;
+  int64_t ncell = 0;
+  int g[3] = {0, 0, 0};
 };
 
 __device__ __forceinline__ double knn_sqdist(const double* __restrict__ a, const double* __restrict__ b, int d) {
@@ -235,7 +247,9 @@ __global__ void knn_brute_kernel(const double* __restrict__ coords, const int32_
   for (int64_t i = q_begin + warp; i < q_end; i += nwarps) {
     const int64_t ncand = min(i, end_search_at + 1);
     int32_t* row = nn + (i - row0) * m;
-    if (ncand <= m) {  // Vecchia_utils.cpp:788-813: all predecessors, in index order
+    // Vecchia_utils.cpp:788-813: rows i <= m take all predecessors, in index order. Later rows go through the walk even when
+    // they have exactly m candidates (prediction with m = the number of observed points): distance order.
+    if (i <= m) {
       for (int p = lane; p < m; p += 32) row[p] = p < ncand ? p : -1;
       continue;
     }
@@ -330,6 +344,57 @@ __global__ void knn_grid_kernel(const double* __restrict__ coords, const int32_t
   }
 }
 
+// First query of the cell-list search: queries with few candidates (the first points of the ordering; every query when there are
+// few observed points, or in more than three dimensions) are done by brute force.
+inline int64_t knn_brute_end(int64_t n, int d, int64_t end_search_at) {
+  if (d > 3 || end_search_at + 1 <= 4096) return n;
+  return std::min<int64_t>(n, 4096);
+}
+
+// Cell grid over the bounding box of all n points (d <= 3), about n / 8 cells of edge h. Only axes at least as wide as a cell are
+// sliced: h is computed from the product of the sliced extents, every axis thinner than h becomes a single slab (g = 1,
+// inv_h = 0, like an axis of zero extent), and h is recomputed until no axis is dropped. Otherwise a thin but non-zero axis (a
+// nearly flat cloud) would shrink the cells along every axis: billions of cells, and neighbours hundreds of rings apart. The
+// widest axis is never dropped, every sliced axis has g <= 2 extent / h, so there are at most 2^d n / 8 cells. Unscanned cells
+// differ from the query's cell along a sliced axis, so the ring stop test of knn_grid_kernel stays valid. Returns the cell count.
+inline int64_t knn_grid_setup(const double* coords_host, int64_t n, int d, KnnGrid* gr) {
+  gr->dim = d;
+  double lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
+  for (int k = 0; k < d; ++k) { lo[k] = coords_host[k]; hi[k] = coords_host[k]; }
+  for (int64_t i = 0; i < n; ++i)
+    for (int k = 0; k < d; ++k) {
+      const double v = coords_host[i * d + k];
+      lo[k] = std::min(lo[k], v); hi[k] = std::max(hi[k], v);
+    }
+  bool sliced[3] = {false, false, false};
+  for (int k = 0; k < d; ++k) sliced[k] = hi[k] > lo[k];
+  const double target_cells = std::max(1.0, (double)n / 8.0);
+  double h = 1.0;
+  for (bool dropped = true; dropped;) {
+    double vol = 1.;
+    int active = 0;
+    for (int k = 0; k < d; ++k) { if (sliced[k]) { vol *= (hi[k] - lo[k]); ++active; } }
+    h = active > 0 ? std::pow(vol / target_cells, 1.0 / active) : 1.0;
+    if (!(h > 0.)) h = 1.0;
+    dropped = false;
+    for (int k = 0; k < d; ++k)
+      if (sliced[k] && hi[k] - lo[k] < h) { sliced[k] = false; dropped = true; }
+  }
+  int64_t ncell = 1;
+  gr->hmin = h;
+  for (int k = 0; k < 3; ++k) {
+    if (k < d && sliced[k]) {
+      int gk = (int)std::min<double>(std::ceil((hi[k] - lo[k]) / h), 1 << 20);
+      gk = std::max(gk, 1);
+      gr->g[k] = gk; gr->lo[k] = lo[k]; gr->inv_h[k] = 1.0 / h;
+    } else {
+      gr->g[k] = 1; gr->lo[k] = k < d ? lo[k] : 0.; gr->inv_h[k] = 0.;  // thin or degenerate axis: one slab
+    }
+    ncell *= gr->g[k];
+  }
+  return ncell;
+}
+
 // Returns the number of kernels launched, or -1 with *err set. coords: device n x d row-major (Vecchia order; prediction: the
 // observed points followed by the prediction points). Queries are the points [q_begin, n); the candidates of query i are the
 // points below min(i, end_search_at + 1); nn_dev holds the rows of the queries only (row of query i = i - q_begin).
@@ -337,7 +402,7 @@ __global__ void knn_grid_kernel(const double* __restrict__ coords, const int32_t
 template <int KS>
 inline int knn_vecchia_device_ks(const double* coords_dev, const double* coords_host, int64_t n, int d, int m,
                                  const int32_t* pos_dev, const int32_t* sort_sum_dev, const double* csum_dev, int32_t* nn_dev,
-                                 cudaStream_t stream, int num_sms, int* num_replayed, std::string* err, int64_t q_begin,
+                                 cudaStream_t stream, int num_sms, KnnInfo* info, std::string* err, int64_t q_begin,
                                  int64_t end_search_at) {
   const int64_t row0 = q_begin;
   auto ck = [&](cudaError_t e, const char* what) {
@@ -357,15 +422,14 @@ inline int knn_vecchia_device_ks(const double* coords_dev, const double* coords_
       int nf = 0;
       if (ok) ok = ck(cudaMemcpyAsync(&nf, nflag, sizeof(int), cudaMemcpyDeviceToHost, stream), "memcpy");
       if (ok) ok = ck(cudaStreamSynchronize(stream), "knn sync");
-      if (num_replayed) *num_replayed = nf;
+      info->replayed = nf;
     }
+    info->launches = launches;
     cudaFree(flagged); cudaFree(nflag);
     return ok ? launches : -1;
   };
-  // queries with few candidates (the first points of the ordering; every query when there are few observed points, or in more
-  // than three dimensions) are done by brute force
-  int64_t brute_end = std::min<int64_t>(n, d <= 3 ? 4096 : n);
-  if (end_search_at + 1 <= 4096) brute_end = n;
+  const int64_t brute_end = knn_brute_end(n, d, end_search_at);
+  info->brute_end = brute_end;
   if (brute_end > q_begin) {
     const int blocks = (int)std::min<int64_t>((brute_end - q_begin + 7) / 8, (int64_t)num_sms * 8);
     knn_brute_kernel<KS><<<std::max(blocks, 1), 256, 0, stream>>>(coords_dev, pos_dev, csum_dev, d, m, q_begin, brute_end, end_search_at, row0,
@@ -376,32 +440,9 @@ inline int knn_vecchia_device_ks(const double* coords_dev, const double* coords_
   if (brute_end >= n) return finish(true);
   // ---- cell list over all points (host computes the bounding box: one pass over n x d doubles)
   KnnGrid gr;
-  gr.dim = d;
-  double vol = 1.;
-  double lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
-  for (int k = 0; k < d; ++k) { lo[k] = coords_host[k]; hi[k] = coords_host[k]; }
-  for (int64_t i = 0; i < n; ++i)
-    for (int k = 0; k < d; ++k) {
-      const double v = coords_host[i * d + k];
-      lo[k] = std::min(lo[k], v); hi[k] = std::max(hi[k], v);
-    }
-  int active = 0;
-  for (int k = 0; k < d; ++k) { if (hi[k] > lo[k]) { vol *= (hi[k] - lo[k]); ++active; } }
-  const double target_cells = std::max(1.0, (double)n / 8.0);
-  double h = active > 0 ? std::pow(vol / target_cells, 1.0 / active) : 1.0;
-  if (!(h > 0.)) h = 1.0;
-  int64_t ncell = 1;
-  gr.hmin = h;
-  for (int k = 0; k < 3; ++k) {
-    if (k < d && hi[k] > lo[k]) {
-      int gk = (int)std::min<double>(std::ceil((hi[k] - lo[k]) / h), 1 << 20);
-      gk = std::max(gk, 1);
-      gr.g[k] = gk; gr.lo[k] = lo[k]; gr.inv_h[k] = 1.0 / h;
-    } else {
-      gr.g[k] = 1; gr.lo[k] = k < d ? lo[k] : 0.; gr.inv_h[k] = 0.;  // degenerate axis: one slab
-    }
-    ncell *= gr.g[k];
-  }
+  const int64_t ncell = knn_grid_setup(coords_host, n, d, &gr);
+  info->ncell = ncell;
+  for (int k = 0; k < 3; ++k) info->g[k] = gr.g[k];
   if (ncell >= ((int64_t)1 << 31)) { *err = "cell grid too large"; return finish(false); }
   uint32_t *cell = nullptr, *cell_sorted = nullptr;
   int32_t *idx = nullptr, *idx_sorted = nullptr, *cell_start = nullptr;
@@ -440,16 +481,50 @@ inline int knn_vecchia_device_ks(const double* coords_dev, const double* coords_
   return rc;
 }
 
-inline int knn_vecchia_device(const double* coords_dev, const double* coords_host, int64_t n, int d, int m,
-                              const int32_t* pos_dev, const int32_t* sort_sum_dev, const double* csum_dev, int32_t* nn_dev,
-                              cudaStream_t stream, int num_sms, int* num_replayed, std::string* err, int64_t q_begin = 0,
-                              int64_t end_search_at = -1) {
-  if (end_search_at < 0) end_search_at = n - 2;
-  if (m <= 32)
-    return knn_vecchia_device_ks<1>(coords_dev, coords_host, n, d, m, pos_dev, sort_sum_dev, csum_dev, nn_dev, stream, num_sms, num_replayed, err,
-                                    q_begin, end_search_at);
-  return knn_vecchia_device_ks<2>(coords_dev, coords_host, n, d, m, pos_dev, sort_sum_dev, csum_dev, nn_dev, stream, num_sms, num_replayed, err,
+// The whole search from host coordinates: coordinate sums and their ranks on the host, then the device kernels. coords_dev and
+// coords_host hold the same n x d row-major points. Model queries: q_begin = 0, end_search_at = n - 2; prediction: q_begin =
+// end_search_at + 1 = the number of observed points. m must not exceed end_search_at + 1 (the caller clips it, :752-755).
+// Returns the number of kernels launched, or -1 with *err set; synchronises `stream`.
+inline int knn_vecchia_search(const double* coords_dev, const double* coords_host, int64_t n, int d, int m, int32_t* nn_dev,
+                              cudaStream_t stream, int num_sms, KnnInfo* info, std::string* err, int64_t q_begin,
+                              int64_t end_search_at) {
+  // rank of every point in the sorted coordinate sums (Vecchia_utils.cpp:775-786). The permutation of equal sums is whatever
+  // std::sort yields, so the same library call is made on the same input.
+  std::vector<double> csum((size_t)n);
+  for (int64_t i = 0; i < n; ++i) {
+    double sacc = 0.;
+    for (int k = 0; k < d; ++k) sacc += coords_host[i * d + k];
+    csum[(size_t)i] = sacc;
+  }
+  std::vector<int> sort_sum((size_t)n);
+  std::iota(sort_sum.begin(), sort_sum.end(), 0);
+  std::sort(sort_sum.begin(), sort_sum.end(), [&csum](int i1, int i2) { return csum[i1] < csum[i2]; });
+  std::vector<int32_t> pos((size_t)n);
+  for (int64_t r = 0; r < n; ++r) pos[(size_t)sort_sum[(size_t)r]] = (int32_t)r;
+  int32_t *pos_dev = nullptr, *sort_sum_dev = nullptr;
+  double* csum_dev = nullptr;
+  cudaError_t e = cudaMalloc(&pos_dev, sizeof(int32_t) * n);
+  if (e == cudaSuccess) e = cudaMalloc(&sort_sum_dev, sizeof(int32_t) * n);
+  if (e == cudaSuccess) e = cudaMalloc(&csum_dev, sizeof(double) * n);
+  if (e == cudaSuccess) e = cudaMemcpy(pos_dev, pos.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(sort_sum_dev, sort_sum.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(csum_dev, csum.data(), sizeof(double) * n, cudaMemcpyHostToDevice);
+  int rc = -1;
+  if (e != cudaSuccess) {
+    *err = std::string("upload: ") + cudaGetErrorString(e);
+  } else if (m <= 32) {
+    rc = knn_vecchia_device_ks<1>(coords_dev, coords_host, n, d, m, pos_dev, sort_sum_dev, csum_dev, nn_dev, stream, num_sms, info, err,
                                   q_begin, end_search_at);
+  } else {
+    rc = knn_vecchia_device_ks<2>(coords_dev, coords_host, n, d, m, pos_dev, sort_sum_dev, csum_dev, nn_dev, stream, num_sms, info, err,
+                                  q_begin, end_search_at);
+  }
+  if (rc >= 0) {
+    e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) { *err = std::string("knn sync: ") + cudaGetErrorString(e); rc = -1; }
+  }
+  cudaFree(pos_dev); cudaFree(sort_sum_dev); cudaFree(csum_dev);
+  return rc;
 }
 
 }  // namespace gpb

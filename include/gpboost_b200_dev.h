@@ -118,6 +118,15 @@ GPBDEV_EXPORT int64_t gpbdev_vecchia_launch_count(gpbdev_vecchia_t h);
 /* number of queries of the device neighbour search that were re-derived by the exact replay of the reference's
  * pruned walk (rounding-decided ties, typically only on lattice data) */
 GPBDEV_EXPORT int gpbdev_vecchia_knn_replayed(gpbdev_vecchia_t h);
+/* Read-back of the device neighbour search, for tests (off the hot path; stateless). coords_host: n x d row-major in the search
+ * order. Model queries (the sets of gpbdev_vecchia_create): q_begin = 0, end_search_at = n - 2. Prediction queries (the sets of
+ * gpbdev_vecchia_predict, observed points first): q_begin = number of observed points, end_search_at = q_begin - 1. m is clipped
+ * to end_search_at + 1 like the reference (Vecchia_utils.cpp:752-755); nn_host receives (n - q_begin) x m_clipped int32, -1
+ * padded, the row of query i at i - q_begin. info_out[7] = {queries replayed, kernels launched, first query of the cell-list
+ * search (n: brute force only), cell count, g[0], g[1], g[2]} (cells 0 without a grid). Refuses null buffers, dim < 1, m outside
+ * [1, 60], q_begin outside [0, n) and any other end_search_at. */
+GPBDEV_EXPORT int gpbdev_knn_search(int device, const double* coords_host, int64_t n, int d, int m, int64_t q_begin,
+                                    int64_t end_search_at, int32_t* nn_host, int64_t* info_out);
 /* measured FP64 FMA peak (TFLOP/s, 2 flops per FMA) of `device`: a register-only DFMA microbenchmark.
  * The Vecchia factor kernel is FP64-pipe bound (SURVEY §8d), so this is its roofline denominator. */
 /* Device collective hook (multi-GPU): in-place sum over all ranks of `count` fp64 values at DEVICE pointer `dev_buf`, enqueued on

@@ -30,23 +30,25 @@ def _cov(cid, dist, var, rt):
 
 def predict_gaussian(coords_obs, y_obs, coords_pred, cov_pars, cov_function="matern", shape=1.5, num_neighbors=20,
                      predict_response=True, num_neighbors_pred=None):
-    """Returns (mean, variance) at coords_pred. cov_pars = (sigma2, sigma1^2, rho) on the original scale. The order of the
-    observed points only matters for distance ties (none for continuous random coordinates). The number of neighbours used
-    for prediction defaults to TWICE the model's num_neighbors (re_model_template.h:299)."""
+    """Returns (mean, variance) at coords_pred. cov_pars = (sigma2, sigma1^2, rho) on the original scale. The neighbour sets
+    come from the reference's walk over the observed points followed by the prediction points (find_nearest_neighbors_Vecchia_fast
+    with start_at = end_search_at + 1 = n, Vecchia_utils.cpp:1784-1800), so distance ties are broken as the reference breaks them
+    when coords_obs is in the model's Vecchia order (the order only matters for ties). The number of neighbours used for
+    prediction defaults to TWICE the model's num_neighbors (re_model_template.h:299)."""
     if num_neighbors_pred is None:
         num_neighbors_pred = 2 * int(num_neighbors)
     num_neighbors = num_neighbors_pred
     coords_obs = np.asarray(coords_obs, dtype=np.float64)
     coords_pred = np.asarray(coords_pred, dtype=np.float64)
     n = coords_obs.shape[0]
-    m = min(int(num_neighbors), n)
+    nbs = ov.knn_range(np.concatenate([coords_obs, coords_pred]), int(num_neighbors), n, n - 1)
     s2, pt = ov.transform_cov_pars(cov_pars, cov_function, shape)
     v, rt = float(pt[0]), float(pt[1])
     cid = ov.cov_id(cov_function, shape)
     mu = np.empty(coords_pred.shape[0]); var = np.empty(coords_pred.shape[0])
     for p in range(coords_pred.shape[0]):
         d = np.sqrt(((coords_obs - coords_pred[p]) ** 2).sum(1))
-        nb = np.argsort(d, kind="stable")[:m]
+        nb = nbs[p]
         cn = coords_obs[nb]
         S = _cov(cid, np.sqrt(((cn[:, None, :] - cn[None, :, :]) ** 2).sum(-1)), v, rt)
         np.fill_diagonal(S, v + 1.)  # marginal variance + nugget (transformed scale)

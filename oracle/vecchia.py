@@ -21,6 +21,7 @@ def lib():
         _lib = C.CDLL(build_oracle())
         _lib.orc_vecchia_factor.restype = C.c_int
         _lib.orc_dense_nll.restype = C.c_int
+        _lib.orc_knn_vecchia_range.restype = C.c_int
     return _lib
 
 
@@ -56,6 +57,26 @@ def knn(coords_ordered, m):
     nn = np.empty((n, m), dtype=np.int32)
     lib().orc_knn_vecchia(_p(cm), C.c_int(n), C.c_int(d), C.c_int(m), _p(nn, C.c_int32))
     return nn
+
+
+def knn_range(coords, m, start_at, end_search_at):
+    """The reference's search for the queries [start_at, n) of coords (n, d), candidates below min(i, end_search_at + 1).
+    Model: start_at = 0, end_search_at = n - 2; prediction (observed points first): start_at = end_search_at + 1 = n_obs.
+    m is clipped to end_search_at + 1. Returns int32 (n - start_at, m_clipped), -1 padded."""
+    n, d = coords.shape
+    cm = np.asfortranarray(coords, dtype=np.float64)
+    nn = np.empty((n - start_at, m), dtype=np.int32)
+    mc = lib().orc_knn_vecchia_range(_p(cm), C.c_int(n), C.c_int(d), C.c_int(m), C.c_int(start_at), C.c_int(end_search_at),
+                                     _p(nn, C.c_int32))
+    return np.ascontiguousarray(nn[:, :mc])
+
+
+def sort_indices(v):
+    """Indices sorting v ascending, by the same std::sort call as the reference (ties in its order)."""
+    v = np.ascontiguousarray(v, dtype=np.float64)
+    out = np.empty(v.shape[0], dtype=np.int32)
+    lib().orc_sort_indices(_p(v), C.c_int(v.shape[0]), _p(out, C.c_int32))
+    return out
 
 
 def factor(coords_ordered, nn, cid, pars_trans, calc_grad=False):

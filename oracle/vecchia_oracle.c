@@ -76,12 +76,20 @@ static void orc_sort_increasing(double* a, int* b, int n) {
 void orc_sort_indices(const double* v, int n, int32_t* idx_out);
 
 /* ---- Vecchia neighbour search among previously ordered points ("nearest" selection):
- * src/GPBoost/Vecchia_utils.cpp:733-985 (driver) and :1029-1093 (find_nearest_neighbors_fast_internal).
- * coords: column-major n x d (already in Vecchia order). nn: n x m int32, -1 padded.
+ * src/GPBoost/Vecchia_utils.cpp:733-985 (driver, CPU branch) and :1029-1093 (find_nearest_neighbors_fast_internal).
+ * coords: column-major n x d (already in Vecchia order). Queries are the points i in [start_at, n); the candidates of query i
+ * are the points c < i with c <= end_search_at (end_search_at < 0: n - 2, :752-754). Model: start_at = 0; prediction (observed
+ * points first, then the prediction points): start_at = end_search_at + 1 = number of observed points.
+ * The neighbour count is clipped to end_search_at + 1 (:755-758); the clipped count is returned. nn: (n - start_at) rows of
+ * stride m, row of query i at i - start_at; the first (clipped) entries of a row hold its neighbours, the rest is -1.
  * The coordinate sums are sorted by the same std::sort call as the reference (orc_sort_indices), because the
  * order of equal sums decides which of several equidistant candidates is met first (lattice data). */
-void orc_knn_vecchia(const double* coords, int n, int d, int m, int32_t* nn) {
-  for (size_t t = 0; t < (size_t)n * m; ++t) nn[t] = -1;
+int orc_knn_vecchia_range(const double* coords, int n, int d, int m, int start_at, int end_search_at, int32_t* nn) {
+  const int ld = m;
+  for (size_t t = 0; t < (size_t)(n - start_at) * ld; ++t) nn[t] = -1;
+  if (end_search_at < 0) end_search_at = n - 2; /* :752-754 */
+  if (m > end_search_at + 1) m = end_search_at + 1; /* :755-758 */
+  if (m < 1) return m;
   double* csum = (double*)malloc(sizeof(double) * n);
   int32_t* sort_sum = (int32_t*)malloc(sizeof(int32_t) * n);
   int* sort_inv = (int*)malloc(sizeof(int) * n);
@@ -92,16 +100,16 @@ void orc_knn_vecchia(const double* coords, int n, int d, int m, int32_t* nn) {
   }
   orc_sort_indices(csum, n, sort_sum);
   for (int i = 0; i < n; ++i) sort_inv[sort_sum[i]] = i;
-  int end_search_at = n - 2; /* :752-754 */
-  /* :788-813 the first m+1 points condition on all predecessors, in index order */
-  for (int i = 1; i < n && i <= m; ++i)
-    for (int j = 0; j < i; ++j) nn[(size_t)i * m + j] = j;
+  /* :788-813 rows 0 < i <= m condition on all predecessors, in index order */
+  for (int i = start_at; i < n && i <= m; ++i)
+    for (int j = 0; j < i; ++j) nn[(size_t)(i - start_at) * ld + j] = j;
+  const int first_i = start_at <= m ? m + 1 : start_at; /* :885 */
 #pragma omp parallel
   {
     double* sq = (double*)malloc(sizeof(double) * m);
 #pragma omp for schedule(dynamic, 256)
-    for (int i = m + 1; i < n; ++i) { /* :885-900 */
-      int32_t* nb = nn + (size_t)i * m;
+    for (int i = first_i; i < n; ++i) { /* :885-900 */
+      int32_t* nb = nn + (size_t)(i - start_at) * ld;
       for (int j = 0; j < m; ++j) sq[j] = INFINITY; /* :1040-1043 */
       int down = 1, up = 1, up_i = sort_inv[i], down_i = sort_inv[i];
       while (up || down) { /* :1049-1092 */
@@ -136,6 +144,12 @@ void orc_knn_vecchia(const double* coords, int n, int d, int m, int32_t* nn) {
     free(sq);
   }
   free(csum); free(sort_sum); free(sort_inv);
+  return m;
+}
+
+/* model queries: n x m */
+void orc_knn_vecchia(const double* coords, int n, int d, int m, int32_t* nn) {
+  orc_knn_vecchia_range(coords, n, d, m, 0, -1, nn);
 }
 
 /* dense Cholesky (lower, in place, row-major ld=m) + solve; stands in for Eigen::LLT at
