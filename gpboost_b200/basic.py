@@ -85,6 +85,8 @@ class GPModel(object):
             (["GP_var", "GP_range"] if self.num_gp else [])
         self.params = dict(_DEFAULT_PARAMS)
         self.num_coef = 0
+        self.num_covariates = 0
+        self.has_covariates = False
         if self.num_gp:
             self._coords_c = np.asfortranarray(gp_coords)  # column-major, gp_coords_data[j*num_data+i]
             coords_ptr = _dptr(self._coords_c)
@@ -123,7 +125,18 @@ class GPModel(object):
                 if k in ("optimizer_cov", "init_cov_pars", "maxit", "delta_rel_conv", "lr_cov", "trace",
                          "convergence_criterion", "m_lbfgs", "estimate_cov_par_index", "std_dev", "cg_max_num_it",
                          "cg_max_num_it_tridiag", "cg_delta_conv", "num_rand_vec_trace", "seed_rand_vec_trace",
-                         "cg_preconditioner_type", "delta_conv_mode_finding"):
+                         "cg_preconditioner_type", "delta_conv_mode_finding", "optimizer_coef",
+                         "init_coef_aux_pars_from_iid_model"):
+                    self.params[k] = v
+                elif k == "init_coef":
+                    if v is None:
+                        self.params[k] = None
+                        continue
+                    v = _as_1d(v, "init_coef")
+                    if self.num_coef == 0:  # basic.py:5335-5344
+                        self.num_coef = v.shape[0]
+                    if v.shape[0] != self.num_coef:
+                        raise ValueError("params['init_coef'] does not contain the correct number of parameters")
                     self.params[k] = v
                 else:
                     raise ValueError("Unknown or unsupported parameter: %s" % k)
@@ -132,6 +145,11 @@ class GPModel(object):
             self._init_cov = _as_1d(self.params["init_cov_pars"], "init_cov_pars", self.num_cov_pars)
             init_c = _dptr(self._init_cov)
         opt_c = c_str(self.params["optimizer_cov"]) if self.params["optimizer_cov"] is not None else None
+        init_coef_c = None
+        if self.params["init_coef"] is not None:
+            self._init_coef = _as_1d(self.params["init_coef"], "init_coef", self.num_coef)
+            init_coef_c = _dptr(self._init_coef)
+        opt_coef_c = c_str(self.params["optimizer_coef"]) if self.params["optimizer_coef"] is not None else None
         est = self.params["estimate_cov_par_index"]
         est = np.full(self.num_cov_pars, -1, dtype=np.int32) if est is None else np.ascontiguousarray(est, dtype=np.int32)
         self._safe_call(self._LIB.GPB_SetOptimConfig(
@@ -139,8 +157,8 @@ class GPModel(object):
             ctypes.c_int(self.params["maxit"]), ctypes.c_double(self.params["delta_rel_conv"]),
             ctypes.c_bool(self.params["use_nesterov_acc"]), ctypes.c_int(self.params["nesterov_schedule_version"]),
             ctypes.c_bool(self.params["trace"]), opt_c, ctypes.c_int(self.params["momentum_offset"]),
-            c_str(self.params["convergence_criterion"]), ctypes.c_int(self.num_coef), None,
-            ctypes.c_double(self.params["lr_coef"]), ctypes.c_double(self.params["acc_rate_coef"]), None,
+            c_str(self.params["convergence_criterion"]), ctypes.c_int(self.num_coef), init_coef_c,
+            ctypes.c_double(self.params["lr_coef"]), ctypes.c_double(self.params["acc_rate_coef"]), opt_coef_c,
             ctypes.c_int(self.params["cg_max_num_it"]), ctypes.c_int(self.params["cg_max_num_it_tridiag"]),
             ctypes.c_double(self.params["cg_delta_conv"]), ctypes.c_int(self.params["num_rand_vec_trace"]),
             ctypes.c_bool(self.params["reuse_rand_vec_trace"]),
@@ -153,19 +171,39 @@ class GPModel(object):
         return self
 
     def fit(self, y, X=None, params=None, offset=None, fixed_effects=None):
-        """Find the covariance parameters that minimise the negative log-likelihood (GPModel.fit, basic.py:5394)."""
-        if X is not None:
-            raise ValueError("Linear fixed effects 'X' are not supported by gpboost_b200.GPModel yet")
+        """Find the covariance parameters that minimise the negative log-likelihood (GPModel.fit, basic.py:5394); with covariates
+        `X` (n x p) also the linear regression coefficients, profiled out by GLS in every evaluation (basic.py:5590-5627)."""
         if offset is None:
             offset = fixed_effects
         y = _as_1d(y, "y", self.num_data)
+        X_c = None
+        if X is not None:
+            X = np.asarray(X, dtype=np.float64)
+            if X.ndim == 1:
+                X = X.reshape(-1, 1)
+            if X.ndim != 2 or X.shape[0] != self.num_data:
+                raise GPBoostError("Incorrect number of data points in X")
+            self.num_covariates = X.shape[1]
+            self.num_coef = self.num_covariates
+            self._X_c = np.ascontiguousarray(X.flatten(order="F"))  # column-major, covariate_data[j*num_data+i]
+            X_c = _dptr(self._X_c)
         self.set_optim_params(params)
         off_c = None
         if offset is not None:
             offset = _as_1d(offset, "offset", self.num_data)
             off_c = _dptr(offset)
-        self._safe_call(self._LIB.GPB_OptimCovPar(self.handle, _dptr(y), off_c))
+        if X is None:
+            self._safe_call(self._LIB.GPB_OptimCovPar(self.handle, _dptr(y), off_c))
+        else:
+            self._safe_call(self._LIB.GPB_OptimLinRegrCoefCovPar(self.handle, _dptr(y), X_c, ctypes.c_int(self.num_covariates), off_c))
+        self.has_covariates = X is not None
         return self
+
+    def get_coef(self, std_err=False):
+        """Linear regression coefficients of the last fit with covariates (GPModel.get_coef, basic.py:6010-6050)."""
+        out = np.zeros(self.num_coef, dtype=np.float64)
+        self._safe_call(self._LIB.GPB_GetCoef(self.handle, _dptr(out), ctypes.c_bool(bool(std_err))))
+        return out
 
     def neg_log_likelihood(self, cov_pars, y, fixed_effects=None):
         """Evaluate the negative log-likelihood at `cov_pars` on the original scale (basic.py:5636-5700)."""
@@ -218,25 +256,34 @@ class GPModel(object):
         return buf.value.decode()
 
     def predict(self, y, gp_coords_pred, cov_pars, predict_var=False, predict_response=True, vecchia_pred_type=None,
-                num_neighbors_pred=-1):
+                num_neighbors_pred=-1, X_pred=None):
         """Predictive mean (and variance) at new locations (GPModel.predict, basic.py:6168-6520 -> GPB_SetPredictionData,
         GPB_PredictREModel), GP part only. Returns dict(mu, var). This library does not export the prediction entries
         yet (SURVEY §8 f1); with `_lib` = the reference library this produces the golden vectors for them."""
         if not hasattr(self._LIB, "GPB_PredictREModel"):
             raise GPBoostError("GPB_PredictREModel is not exported by this library (prediction with the GP part: SURVEY §8 f1, not built yet)")
-        y = _as_1d(y, "y", self.num_data)
+        y_c = None if y is None else _dptr(_as_1d(y, "y", self.num_data))
         Xp = np.asfortranarray(np.asarray(gp_coords_pred, dtype=np.float64))
         npred = Xp.shape[0]
-        cp = _as_1d(cov_pars, "cov_pars", self.num_cov_pars)
+        cp_c = None if cov_pars is None else _dptr(_as_1d(cov_pars, "cov_pars", self.num_cov_pars))
+        xp_c = None
+        if X_pred is not None:  # covariates at the prediction points: X_pred beta is added to the mean (basic.py:6360-6380)
+            X_pred = np.asarray(X_pred, dtype=np.float64)
+            if X_pred.ndim == 1:
+                X_pred = X_pred.reshape(-1, 1)
+            if X_pred.shape[0] != npred:
+                raise GPBoostError("Incorrect number of data points in X_pred")
+            self._Xpred_c = np.ascontiguousarray(X_pred.flatten(order="F"))
+            xp_c = _dptr(self._Xpred_c)
         self._safe_call(self._LIB.GPB_SetPredictionData(
-            self.handle, ctypes.c_int32(npred), None, None, None, _dptr(Xp), None, None,
+            self.handle, ctypes.c_int32(npred), None, None, None, _dptr(Xp), None, xp_c,
             c_str(vecchia_pred_type) if vecchia_pred_type else None, ctypes.c_int(num_neighbors_pred), ctypes.c_double(-1.),
             ctypes.c_int(-1), ctypes.c_int(-1)))
         out = np.zeros(npred * (2 if predict_var else 1), dtype=np.float64)
         self._safe_call(self._LIB.GPB_PredictREModel(
-            self.handle, _dptr(y), ctypes.c_int32(npred), _dptr(out), ctypes.c_bool(False), ctypes.c_bool(predict_var),
+            self.handle, y_c, ctypes.c_int32(npred), _dptr(out), ctypes.c_bool(False), ctypes.c_bool(predict_var),
             ctypes.c_bool(predict_response), ctypes.c_bool(False), ctypes.c_bool(False), ctypes.c_int(0), ctypes.c_int(0),
-            None, None, None, _dptr(Xp), None, _dptr(cp), None, ctypes.c_bool(True), None, None))
+            None, None, None, _dptr(Xp), None, cp_c, xp_c, ctypes.c_bool(True), None, None))
         return {"mu": out[:npred].copy(), "var": out[npred:].copy() if predict_var else None}
 
     # ---- CUDA-build extensions ------------------------------------------------------------------------

@@ -198,6 +198,14 @@ struct gpbdev_vecchia {
   bool grad_stores = true;  // GPB200_GRAD_STORES=0: no STORE shortcut after a gradient pass, no extra stores in that pass
   bool nll1_only = false;   // GPB200_NLL_KERNEL=1: one-observation kernel also at d = 2, 20 < m <= 30
   std::vector<int32_t> nn_host;  // kept for the lazy CSC build
+  // linear regression covariates (covariates.cuh), lazy
+  int p = 0;                       // number of covariates
+  double* X = nullptr;             // n x p ROW-major, Vecchia order
+  double* y0 = nullptr;            // n: y - offset, Vecchia order (the response is the residual y0 - X beta)
+  double* gram_partial = nullptr;  // gram_chunks x (p^2 + p)
+  double* gram_out = nullptr;      // p^2 + p
+  double* quad_partial = nullptr;  // per-warp sums of the residual pass
+  int gram_chunks = 0;
 };
 
 namespace {
@@ -464,6 +472,7 @@ int gpbdev_vecchia_free(gpbdev_vecchia_t h) {
   cudaFree(h->dA); cudaFree(h->dD);
   cudaFree(h->A); cudaFree(h->Dinv); cudaFree(h->u); cudaFree(h->yaux); cudaFree(h->colptr); cudaFree(h->csc_pos);
   cudaFree(h->csc_row); cudaFree(h->A_csc);
+  cudaFree(h->X); cudaFree(h->y0); cudaFree(h->gram_partial); cudaFree(h->gram_out); cudaFree(h->quad_partial);
   cudaFree(h->partials); cudaFree(h->sums); cudaFree(h->flush);
   cudaFreeHost(h->sums_host); cudaFreeHost(h->stage_host);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -773,4 +782,5 @@ int gpbdev_vecchia_flush_l2(gpbdev_vecchia_t h) {
 }  // extern "C"
 
 #include "newton.cuh"
+#include "covariates.cuh"
 #include "laplace.cuh"

@@ -44,19 +44,6 @@ int GPB_GetAuxPars(REModelHandle handle, double* aux_pars, char* out_str, bool c
   API_END();
 }
 
-int GPB_GetCoef(REModelHandle handle, double* optim_coef, bool calc_std_dev) {
-  API_BEGIN();
-  (void)handle; (void)optim_coef; (void)calc_std_dev;
-  Unsupported("GPB_GetCoef");
-  API_END();
-}
-
-int GPB_GetCovariateData(REModelHandle handle, double* covariate_data) {
-  API_BEGIN();
-  (void)handle; (void)covariate_data;
-  Unsupported("GPB_GetCovariateData");
-  API_END();
-}
 
 int GPB_GetInitAuxPars(REModelHandle handle, double* aux_pars) {
   API_BEGIN();

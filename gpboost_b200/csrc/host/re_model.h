@@ -39,6 +39,17 @@ class REModel {
                       const int* estimate_cov_par_index);
 
   // iterative-method settings of GPB_SetOptimConfig consumed by the Laplace-Vecchia path (re_model_template.h:860-900)
+  // coefficient fields of GPB_SetOptimConfig (re_model.cpp:318-345): init_coef (num_covariates values or nullptr), optimizer_coef
+  // (only "wls", the Gaussian default, or unset) and init_coef_aux_pars_from_iid_model
+  void SetCoefOptimConfig(int num_covariates, const double* init_coef, const char* optimizer_coef, bool init_coef_from_iid_model);
+  // REModel::OptimLinRegrCoefCovPar (re_model.cpp:548-625) for the Gaussian Vecchia model: covariance parameters by L-BFGS with the
+  // linear regression coefficients profiled out by GLS in every evaluation (ProfileOutCoef, re_model_template.h:2665-2683).
+  // covariate_data: num_data x num_covariates column-major, 1 <= num_covariates <= 64.
+  void OptimLinRegrCoefCovPar(const double* y_data, const double* covariate_data, int num_covariates, const double* fixed_effects);
+  // GPB_GetCoef / GPB_GetCovariateData (column-major num_data x num_covariates)
+  void GetCoef(double* out, bool calc_std_dev) const;
+  void GetCovariateData(double* out) const;
+  int NumCovariates() const { return num_covariates_; }
   void SetIterativeConfig(int cg_max_num_it, int cg_max_num_it_tridiag, double cg_delta_conv, int num_rand_vec_trace,
                           const char* cg_preconditioner_type, int seed_rand_vec_trace, double delta_conv_mode_finding);
   // REModel::OptimCovPar (re_model.cpp:483-541)
@@ -60,12 +71,14 @@ class REModel {
   // gradient of the tree that was just grown stay in HBM; only the L x L system comes to the host. After CalcGradient*.
   void NewtonUpdateLeafValuesDevice(const int32_t* leaf_of_row_dev, int num_leaves, const double* grad_dev, double* leaf_values);
   // GPB_SetPredictionData (c_api.h:1601-1613): prediction locations / neighbour count kept for later Predict calls
-  void SetPredictionData(int32_t num_data_pred, const double* gp_coords_data_pred, const char* vecchia_pred_type, int num_neighbors_pred);
+  // covariate_data_pred: num_data_pred x num_covariates column-major, required exactly when the model has covariates
+  void SetPredictionData(int32_t num_data_pred, const double* gp_coords_data_pred, const double* covariate_data_pred,
+                         const char* vecchia_pred_type, int num_neighbors_pred);
   // REModel::Predict (re_model.cpp:1081-1215) for the Gaussian Vecchia model (SURVEY §8 f1): out_predict = mean (num_data_pred),
   // followed by the predictive variances when predict_var. gp_coords_data_pred column-major like every matrix of the API.
   void Predict(const double* y_obs, int32_t num_data_pred, double* out_predict, bool predict_cov_mat, bool predict_var,
                bool predict_response, const double* gp_coords_data_pred, const double* cov_pars_pred, bool use_saved_data,
-               const double* fixed_effects);
+               const double* fixed_effects, const double* covariate_data_pred = nullptr);
   // GPB_GetCovPar / GPB_GetInitCovPar (original scale)
   void GetCovPar(double* out, bool calc_std_dev) const;
   void GetInitCovPar(double* out) const;
@@ -92,12 +105,17 @@ class REModel {
   // one device pass at transformed (var, range); fills sums_
   void DevicePass(double var, double range, int mode);
   double NegLLFromSums(double sigma2) const;
+  // STORE pass at (var, range), G = X^T Psi^-1 X and r = X^T Psi^-1 (y - offset) on the device, coef_ = G^-1 r, then the residual
+  // y - offset - X coef_ becomes the engine's response; sums_ QUAD / LOGDET / NBAD belong to the residual
+  void ProfileOutCoef(double var, double range);
+  void InitCoefFromIidModel(const double* y_data, const double* fixed_effects);
 
   int32_t num_data_ = 0;
   int dim_ = 0;
   int num_neighbors_ = 20;
   int num_neighbors_pred_ = 40;          // 2 x num_neighbors (re_model_template.h:299)
   std::vector<double> coords_pred_saved_;  // np x d row-major (GPB_SetPredictionData)
+  std::vector<double> covariates_pred_saved_;  // np x num_covariates column-major (GPB_SetPredictionData)
   int32_t num_data_pred_saved_ = 0;
   bool y_has_been_set_ = false;
   int cov_id_ = 0;
@@ -152,6 +170,15 @@ class REModel {
   std::vector<int> estimate_cov_par_index_;
   LbfgsMemory lbfgs_mem_;
   bool cov_pars_estimated_once_ = false;
+
+  // linear regression coefficients (OptimLinRegrCoefCovPar)
+  int num_covariates_ = 0;
+  std::vector<double> X_;          // num_data x num_covariates column-major, original order (GPB_GetCovariateData)
+  std::vector<double> coef_;       // current coefficients
+  std::vector<double> init_coef_;  // GPB_SetOptimConfig init_coef
+  bool init_coef_given_ = false;
+  bool init_coef_from_iid_model_ = true;
+  std::string optimizer_coef_;     // GPB_SetOptimConfig optimizer_coef ("" = unset), checked by a fit with covariates
 };
 
 }  // namespace gpb200

@@ -101,6 +101,18 @@ GPBDEV_EXPORT int gpbdev_vecchia_predict(gpbdev_vecchia_t h, int cov_type, doubl
  * and g = grad_dev (n doubles, original order, device). The caller solves M x = -sigma^2 rhs (L <= 256). */
 GPBDEV_EXPORT int gpbdev_vecchia_newton_system(gpbdev_vecchia_t h, const int32_t* leaf_of_row_dev, int num_leaves, const double* grad_dev,
                                                double* M_host, double* rhs_host);
+/* Linear regression coefficients of the Gaussian Vecchia model, profiled out by GLS (ProfileOutCoef / UpdateCoefGLS,
+ * include/GPBoost/re_model_template.h:2665-2683, :10012-10019). Whole-model engines only (row-sharded engines are refused).
+ * set_covariates: X_colmajor_host is n x p COLUMN-major in the original observation order (as the C API delivers it), 1 <= p <= 64;
+ * it is kept on the device row-major in Vecchia order. The engine's current response (gpbdev_vecchia_set_y: y - offset) is kept
+ * as y0, the fixed part of every residual. */
+GPBDEV_EXPORT int gpbdev_vecchia_set_covariates(gpbdev_vecchia_t h, const double* X_colmajor_host, int p);
+/* After a STORE eval at theta: G_host (p x p row-major, symmetric) = X^T Psi^-1 X and r_host (p) = X^T Psi^-1 y0, summed in a
+ * fixed order (two calls give bitwise the same result). */
+GPBDEV_EXPORT int gpbdev_vecchia_gls_gram(gpbdev_vecchia_t h, double* G_host, double* r_host);
+/* After a STORE eval: installs y_r = y0 - X beta_host as the engine's response and recomputes u = D^-1 B y_r from the resident
+ * factor (no covariance evaluation). out3 = { y_r^T Psi^-1 y_r, log|Psi|, #(D_i <= 0) } (GPBDEV_SUM_QUAD.._NBAD). */
+GPBDEV_EXPORT int gpbdev_vecchia_gls_residual(gpbdev_vecchia_t h, const double* beta_host, double* out3);
 /* Latent factor (non-Gaussian likelihood) and its derivative w.r.t. log(range) — B_grad[1] = -dA, D_grad[1] = dD of
  * CalcCovFactorGradientVecchia (src/GPBoost/Vecchia_utils.cpp:1636-1652) — copied to host buffers (A, dA: n x m row-major in
  * Vecchia order; Dinv, dD: n). Diagnostics / test entry of the factor kernel's MODE_STORE_GRAD. */
