@@ -14,7 +14,7 @@ extern "C" void GPB200_SetLastErrorMessage(const char* msg);
 namespace {
 [[noreturn]] void Unsupported(const char* entry) {
   throw std::runtime_error(std::string(entry) + " is outside the hot path this build carries (SURVEY §8): Vecchia / exact / "
-                           "single-level grouped models with the Gaussian or bernoulli_logit likelihood, L2 tree boosting on dense numerical features");
+                           "single-level grouped models with the gaussian, bernoulli_logit or poisson likelihood, L2 tree boosting on dense numerical features");
 }
 inline gpb200::REModel* RM(void* h) {
   if (h == nullptr) throw std::runtime_error("REModel handle is null");
@@ -53,7 +53,7 @@ int GPB_GetInitAuxPars(REModelHandle handle, double* aux_pars) {
 
 int GPB_GetNumAuxPars(BoosterHandle handle, int* num_aux_pars) {
   API_BEGIN();
-  (void)handle; *num_aux_pars = 0;  // gaussian, bernoulli_logit: no auxiliary parameters
+  (void)handle; *num_aux_pars = 0;  // gaussian, bernoulli_logit, poisson: no auxiliary parameters
   API_END();
 }
 

@@ -129,10 +129,13 @@ class REModel {
   gpbdev_grouped_t grouped_ = nullptr;   // single-level grouped random effect backend (SURVEY §8 a7)
   gpbdev_dense_t dense_ = nullptr;       // exact GP backend, gp_approx = "none" (SURVEY §8 a6)
   void DensePass(double var, double range, bool with_grad = false);
-  // non-Gaussian likelihood (bernoulli_logit) with a latent Vecchia GP: Laplace approximation on the device (SURVEY §8 a12)
+  // non-Gaussian likelihood (bernoulli_logit, poisson) with a latent Vecchia GP: Laplace approximation on the device (SURVEY §8 a12)
   bool gauss_ = true;
+  bool poisson_ = false;
   bool device_collective_ = false;  // the engine all-reduces its results itself (NCCL on its stream)
   void EvalLaplace(const double* y_data, const double* cov_pars, double* negll, const double* fixed_effects);
+  // checks poisson labels (non-negative integers) and returns -sum_i log(y_i!)
+  double CheckCountsLogNormConst(const double* y) const;
   void EnsureProbes();
   double TransformRange(double range) const;
   int cg_max_num_it_ = 1000, cg_max_num_it_tridiag_ = 1000, num_rand_vec_trace_ = 50, seed_rand_vec_trace_ = 1;

@@ -150,12 +150,22 @@ GPBDEV_EXPORT int gpbdev_fp64_peak(int device, double* tflops);
 /* write > L2-size bytes to evict the L2 between timed iterations */
 GPBDEV_EXPORT int gpbdev_vecchia_flush_l2(gpbdev_vecchia_t h);
 
-/* ---- Laplace approximation, latent Vecchia GP + bernoulli_logit likelihood (SURVEY §8 a12) -----------------------
+/* ---- Laplace approximation, latent Vecchia GP + bernoulli_logit or poisson likelihood (SURVEY §8 a12) -------------
  * Replaces FindModePostRandEffCalcMLLVecchia (include/GPBoost/likelihoods.h:3773-4059) with
  * matrix_inversion_method = "iterative", cg_preconditioner_type = "vadu": Newton mode finding with PCG solves
  * (CGVecchiaLaplaceVec, src/GPBoost/CG_utils.cpp:21-108) and the log-determinant by stochastic Lanczos quadrature
  * (CalcLogDetStochVecchia likelihoods.h:16376-16521, CGTridiagVecchiaLaplace CG_utils.cpp:110-229).
- * Labels (0/1 as doubles) are set with gpbdev_vecchia_set_y. */
+ * Labels (0/1 or counts, as doubles) are set with gpbdev_vecchia_set_y. */
+/* likelihood of the Laplace engine (bernoulli_logit until set otherwise) */
+enum { GPBDEV_LIK_BERNOULLI_LOGIT = 0, GPBDEV_LIK_POISSON = 1 };
+/* Select the instance of the per-row kernels. log_norm_const is added to every log-likelihood sum of poisson (the reference's
+ * log_normalizing_constant_ = -sum_i log(y_i!), likelihoods.h:10750-10757); it is ignored for bernoulli_logit. */
+GPBDEV_EXPORT int gpbdev_vecchia_laplace_set_likelihood(gpbdev_vecchia_t h, int likelihood, double log_norm_const);
+/* Read-back of the three per-row kernels of one likelihood, for tests (stateless, off the hot path), on `device`, 1 <= n <= 2^20 rows
+ * with loc = mode + fe (fe_host may be NULL). out_host: 5 x n: W, Newton right-hand side, D^-1 + W, the row's log-likelihood term
+ * (without the normalising constant; one warp of row_stats_kernel per row), dW. */
+GPBDEV_EXPORT int gpbdev_laplace_rows(int device, int likelihood, int64_t n, const double* y_host, const double* mode_host,
+                                      const double* fe_host, const double* Dinv_host, double* out_host);
 /* probe vectors r_i ~ N(0, I): n x t COLUMN-major, rows in the Vecchia order (GenRandVecNormalParallel, CG_utils.cpp:978) */
 GPBDEV_EXPORT int gpbdev_vecchia_laplace_set_probes(gpbdev_vecchia_t h, const double* probes_colmajor, int t);
 /* cfg[8]: 0 maxit_mode_newton, 1 delta_conv_mode_finding, 2 max step halvings, 3 cg_max_num_it, 4 cg_max_num_it_tridiag,
