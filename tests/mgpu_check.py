@@ -101,7 +101,7 @@ def main():
                 assert np.max(np.abs(tr["leaf_value"] - np.array(g["leaf_value"]))) <= 1e-8 * np.max(np.abs(g["leaf_value"]))
             assert np.abs(score[:64] - np.array(rec["score_head"])).max() <= 1e-8 * np.abs(rec["score_head"]).max()
             assert abs(score.sum() - rec["score_sum"]) <= 1e-8 * max(abs(rec["score_sum"]), np.abs(score).sum() * 1e-3)
-        log("boosting sharded ok:", spec["name"], os.environ.get("GPB200_SHARDED_LOOP", "device"))
+        log("boosting sharded ok:", spec["name"])
 
     # ---- 3. Laplace-Vecchia with the SLQ probe columns sharded over the ranks
     lg = json.load(open(os.path.join(HERE, "golden", "laplace_golden.json")))["cases"]

@@ -82,43 +82,28 @@ def test_device_tree_matches_oracle(lib, n, F, levels, L, mdl):
         assert np.allclose(d["split_gain"], a["split_gain"], rtol=1e-5)
 
 
-# every implementation of the tree-side kernels that the library carries (environment switches read when a learner is created)
-VARIANTS = {
-    "hist1_scan_cub": {"GPB200_HIST_KERNEL": "1", "GPB200_PARTITION": "1", "GPB200_FUSED_SCAN": "0", "GPB200_TREE_LOOP": "host"},
-    "hist2_part2": {"GPB200_HIST_KERNEL": "2", "GPB200_PARTITION": "2", "GPB200_FUSED_SCAN": "0", "GPB200_TREE_LOOP": "host"},
-    "hist2_part2_fused": {"GPB200_HIST_KERNEL": "2", "GPB200_PARTITION": "2", "GPB200_FUSED_SCAN": "1", "GPB200_TREE_LOOP": "host"},
-    "device_loop": {"GPB200_HIST_KERNEL": "2", "GPB200_PARTITION": "2", "GPB200_FUSED_SCAN": "1", "GPB200_TREE_LOOP": "device"},
-    "graph_loop": {"GPB200_HIST_KERNEL": "2", "GPB200_PARTITION": "2", "GPB200_FUSED_SCAN": "1", "GPB200_TREE_LOOP": "graph"},
-}
+# the two ways the leaf loop is enqueued on one GPU: a replayed graph (device gradients) and eagerly (host gradients); the Booster
+# always passes device gradients (test_booster_matches_reference_golden)
+VARIANTS = {"graph": True, "eager": False}
+VARIANT_CASES = [(30000, 40, 255, 31, 20), (10000, 70, 16, 63, 3), (500, 3, 5, 31, 1), (20000, 9, 2, 16, 50), (50, 2, 4, 4, 30)]
 
 
 @pytest.mark.parametrize("variant", list(VARIANTS))
-def test_tree_kernel_variants_match_oracle(lib, tree_golden, variant, monkeypatch):
-    """Same parity bar for every kernel variant: oracle trees (incl. binary and constant-heavy features, F > 64, a leaf budget
-    the data cannot fill) through gpbdev_tree_train (host gradients, device-resident ones for the graph loop), and one reference
-    golden through the Booster (device-resident gradients). tests/test_tree_kernels_gpu.py covers every kernel combination."""
-    for k, v in VARIANTS[variant].items():
-        monkeypatch.setenv(k, v)
-    for n, F, levels, L, mdl in [(30000, 40, 255, 31, 20), (10000, 70, 16, 63, 3), (500, 3, 5, 31, 1), (20000, 9, 2, 16, 50), (50, 2, 4, 4, 30)]:
-        rng = np.random.default_rng(n + F)
-        bins = rng.integers(0, levels, size=(F, n)).astype(np.uint8)
-        grad = rng.standard_normal(n) + (bins[0] > levels // 2) * 0.8 - (bins[min(1, F - 1)] % 3 == 0) * 0.5
-        cfg = ot.make_config(num_leaves=L, min_data_in_leaf=mdl)
-        a = ot.train_tree(bins, np.full(F, levels), grad, cfg)
-        d = dev_train(lib, bins, np.full(F, levels), grad, cfg, on_device=variant == "graph_loop")
-        assert d["num_leaves"] == a["num_leaves"], (variant, n, F)
-        for k in ("split_feature", "threshold_bin", "left_child", "right_child", "leaf_count"):
-            assert np.array_equal(d[k], a[k]), (variant, n, F, k)
-        if a["num_leaves"] > 1:
-            assert np.max(np.abs(d["leaf_value"] - a["leaf_value"])) <= 1e-10 * np.max(np.abs(a["leaf_value"])), (variant, n, F)
-    rec = [r for r in tree_golden["cases"] if not r["spec"].get("gp")][0]
-    trees, score, _, _, _ = _run_product(rec["spec"])
-    assert len(trees) == len(rec["trees"])
-    for t, g in zip(trees, rec["trees"]):
-        assert np.array_equal(t["split_feature"], np.array(g["split_feature"])) and np.array_equal(t["threshold"], np.array(g["threshold"]))
-        assert np.array_equal(t["leaf_count"], np.array(g["leaf_count"]))
-        assert np.max(np.abs(t["leaf_value"] - np.array(g["leaf_value"]))) <= 1e-10 * np.max(np.abs(g["leaf_value"]))
-    assert abs(score.sum() - rec["score_sum"]) <= 1e-9 * abs(rec["score_sum"])
+@pytest.mark.parametrize("n,F,levels,L,mdl", VARIANT_CASES)
+def test_tree_kernel_variants_match_oracle(lib, variant, n, F, levels, L, mdl):
+    """Same parity bar on both ways of enqueuing the leaf loop: oracle trees (incl. binary and constant-heavy features, F > 64, a
+    leaf budget the data cannot fill) through gpbdev_tree_train. tests/test_tree_kernels_gpu.py covers every path."""
+    rng = np.random.default_rng(n + F)
+    bins = rng.integers(0, levels, size=(F, n)).astype(np.uint8)
+    grad = rng.standard_normal(n) + (bins[0] > levels // 2) * 0.8 - (bins[min(1, F - 1)] % 3 == 0) * 0.5
+    cfg = ot.make_config(num_leaves=L, min_data_in_leaf=mdl)
+    a = ot.train_tree(bins, np.full(F, levels), grad, cfg)
+    d = dev_train(lib, bins, np.full(F, levels), grad, cfg, on_device=VARIANTS[variant])
+    assert d["num_leaves"] == a["num_leaves"], (variant, n, F)
+    for k in ("split_feature", "threshold_bin", "left_child", "right_child", "leaf_count"):
+        assert np.array_equal(d[k], a[k]), (variant, n, F, k)
+    if a["num_leaves"] > 1:
+        assert np.max(np.abs(d["leaf_value"] - a["leaf_value"])) <= 1e-10 * np.max(np.abs(a["leaf_value"])), (variant, n, F)
 
 
 def _run_product(spec):

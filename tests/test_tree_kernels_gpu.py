@@ -1,21 +1,18 @@
-"""Every kernel path of the device tree learner against the tree oracle, at kernel level (C ABI only).
+"""Every path of the device tree learner against the tree oracle, at kernel level (C ABI only).
 
-`gpbdev_tree_train` (gpboost_b200/csrc/dev/tree_api.cu) grows a tree through one of three leaf loops and, inside it, one of
-several separately written kernels, picked from switches read when the learner is created, from num_leaves and from where
-the gradient lives:
+`gpbdev_tree_train` (gpboost_b200/csrc/dev/tree_api.cu) grows every tree through one leaf loop on the device (hist3_kernel,
+reduce_scan2_kernel, tree_advance_kernel, part_count_kernel + part_scatter_kernel per split). It enqueues that loop in one of three
+ways, picked from num_leaves, from where the gradient lives and from whether a collective is installed:
 
-  loop       graph (default): the device-resident loop captured once per (gradient buffer, hessian) and replayed; needs
-             device gradients and num_leaves <= 256 (kMaxLeavesDev)
-             device: the same kernels enqueued eagerly (GPB200_TREE_LOOP=device, or host gradients)
-             host: one device-to-host copy per split (GPB200_TREE_LOOP=host, or num_leaves > 256)
-  histogram  hist_kernel (1, host loop only) / hist2_kernel (2) / hist3_kernel<false> (3, default) / hist3_kernel<true> (4)
-  scan       host loop: hist_reduce_kernel + split_scan_kernel (GPB200_FUSED_SCAN=0) / reduce_scan_kernel (1) / reduce_scan2_kernel (2)
-             device loops: reduce_scan_kernel (0 or 1) / reduce_scan2_kernel (2, default)
-  advance    device loops: tree_advance_kernel (GPB200_FUSED_ADVANCE=1, default) / split_argmax + select + plan kernels (0)
-  partition  host loop: mark + CUB scan + scatter (GPB200_PARTITION=1) / part_count + part_scatter (2, default);
-             device loops always run part_count + part_scatter between the two row-index buffers
+  graph    device gradients and num_leaves <= 256 (one batch of splits): captured once per (gradient buffer, hessian), replayed
+  eager    host gradients, or num_leaves > 256: enqueued in batches of 255 splits; between batches the host reads whether the
+           tree is finished and stops
+  sharded  a data-parallel learner, here one GPU with an identity collective (gpbdev_tree_set_allreduce): the same loop enqueued
+           eagerly with hist_reduce_kernel into the staging histogram, the all-reduce, reduce_scan2_kernel from the stage and the
+           children's local ranges set after the partition (tree_local_ranges_kernel)
 
-test_cases_reach_every_kernel_path checks, without a GPU, that the runs below reach every combination.
+test_cases_reach_every_kernel_path checks, without a GPU, that the runs below reach every path with one batch and with several,
+and a tree that stops in a later batch.
 
 Pass bars against oracle/tree_oracle.c: number of leaves, split features, threshold bins, children, leaf counts and the leaf
 of every row bit-exact; leaf values <= 1e-10 of the largest one (the device merges per-chunk partial sums, the oracle adds row
@@ -29,38 +26,17 @@ import pytest
 
 from oracle import tree as ot
 
-SWITCHES = ("GPB200_TREE_LOOP", "GPB200_HIST_KERNEL", "GPB200_FUSED_SCAN", "GPB200_FUSED_ADVANCE", "GPB200_PARTITION",
-            "GPB200_SHARDED_LOOP")
-MAX_LEAVES_DEV = 256  # kMaxLeavesDev
+SPLIT_BATCH = 255  # kSplitBatch: splits enqueued between two reads of the finished flag; the graph holds one batch
 KEPS = float(np.float32(1e-15))  # kEpsilon
 
 
-def path(env, L, grad_on_device):
-    """(loop, hist, scan, advance, partition) that gpbdev_tree_train runs on one GPU. Restates the switch parsing of
-    tree_create_common, the loop choice of gpbdev_tree_train, the kernel choice of tree_train_device_loop and that of the
-    host-driven loop (build_hist, the fused / unfused scan, the partition versions)."""
-    e = env.get("GPB200_TREE_LOOP")
-    device_loop = 2 if e is None else (1 if e == "device" else (0 if e == "host" else 2))
-    h = int(env.get("GPB200_HIST_KERNEL", "3"))
-    hist = h if 1 <= h <= 4 else 3
-    s = int(env.get("GPB200_FUSED_SCAN", "2"))
-    fused_scan = 0 if s == 0 else (1 if s == 1 else 2)
-    advance = 0 if int(env.get("GPB200_FUSED_ADVANCE", "1")) == 0 else 1
-    partition = 1 if int(env.get("GPB200_PARTITION", "2")) == 1 else 2
-    if device_loop == 2 and L <= MAX_LEAVES_DEV and grad_on_device:
-        loop = "graph"
-    elif device_loop >= 1 and L <= MAX_LEAVES_DEV:
-        loop = "device"
-    else:
-        loop = "host"
-    if loop == "host":
-        return (loop, hist, ("split_scan", "reduce_scan", "reduce_scan2")[fused_scan], None, partition)
-    return (loop, 2 if hist == 1 else hist, "reduce_scan2" if fused_scan == 2 else "reduce_scan", advance, 2)
-
-
-HOST_BUCKETS = {("host", h, s, None, p) for h in (1, 2, 3, 4) for s in ("split_scan", "reduce_scan", "reduce_scan2") for p in (1, 2)}
-DEVICE_BUCKETS = {(loop, h, s, a, 2) for loop in ("device", "graph") for h in (2, 3, 4) for s in ("reduce_scan", "reduce_scan2")
-                  for a in (0, 1)}
+def path(kind, L, on_device):
+    """(leaf loop, batches of splits enqueued for a full tree) that gpbdev_tree_train runs on one GPU; kind "sharded" = an
+    identity collective is installed. Restates the choice in tree_grow."""
+    batches = -(-(L - 1) // SPLIT_BATCH)
+    if kind == "sharded":
+        return "sharded", batches
+    return ("graph" if on_device and batches == 1 else "eager"), batches
 
 
 # ---------------------------------------------------------------------------------------------------------------- data
@@ -170,8 +146,11 @@ GRADS = [(4097, 33, 31, "tiny", False, {}),
          (4097, 33, 31, "int2", True, {"min_data_in_leaf": 1}),
          (4097, 33, 31, "cont", True, {})]
 SPLIT = KNOBS + GRADS
-# leaf budgets: 256 fills the device state, 257 and 300 take the host loop whatever the switches say
-LEAVES = [(4097, 33, L, "grid", False, {"min_data_in_leaf": 3}) for L in (2, 3, 31, 255, 256, 257, 300)]
+# leaf budgets around the batches of 255 splits (256 leaves: the last graph), and one the data cannot fill (the tree stops in a
+# later batch)
+FILLED = (2, 3, 31, 255, 256, 257, 300, 511, 512, 513, 766)
+EARLY_STOP = 2000
+LEAVES = [(4097, 33, L, "grid", False, {"min_data_in_leaf": 3}) for L in FILLED + (EARLY_STOP,)]
 
 
 def stump_gain(bins, num_bin, grad):
@@ -211,41 +190,15 @@ def oracle_config(cfg):
 
 
 # ---------------------------------------------------------------------------------------------------------------- runs
-def _env(loop=None, hist=None, scan=None, advance=None, partition=None):
-    e = {"GPB200_TREE_LOOP": loop, "GPB200_HIST_KERNEL": hist, "GPB200_FUSED_SCAN": scan, "GPB200_FUSED_ADVANCE": advance,
-         "GPB200_PARTITION": partition}
-    return {k: str(v) for k, v in e.items() if v is not None}
-
-
-# (switches, gradient on the device, cases)
-RUNS = []
-for _h in (1, 2, 3, 4):
-    for _s in (0, 1, 2):
-        for _p in (1, 2):
-            RUNS.append((_env("host", _h, _s, None, _p), (_h + _s + _p) % 2, CORE))
-for _loop in ("device", "graph"):
-    for _h in (2, 3, 4):
-        for _s in (1, 2):
-            for _a in (0, 1):
-                RUNS.append((_env(_loop, _h, _s, _a), 1 if _loop == "graph" else (_h + _s + _a) % 2, CORE))
-# the shapes on every histogram kernel (default scan and partition) in the host loop and the graph
-for _h in (1, 2, 3, 4):
-    RUNS.append((_env("host", _h), 1, SHAPES))
-for _h in (2, 3, 4):
-    RUNS.append((_env("graph", _h), 1, SHAPES))
-# the knobs and gradient kinds on every scan implementation; {} = what the library does with no switch set
-RUNS += [({}, 1, SPLIT), ({}, 0, SPLIT), (_env("graph", scan=1), 1, SPLIT), (_env("host", scan=0), 0, SPLIT),
-         (_env("host", scan=1), 1, SPLIT), (_env("host", scan=2), 1, SPLIT)]
-RUNS += [({}, 1, LEAVES), ({}, 0, LEAVES), (_env("host"), 1, LEAVES), (_env("device", hist=4, advance=0), 0, LEAVES)]
-# the default kernels on the shapes with host gradients (eager device loop)
-RUNS.append(({}, 0, SHAPES))
+# (kind, gradient on the device, case): every case set on every kind. "graph" passes device gradients (budgets above 256 leaves
+# then run eagerly from device gradients), "eager" host gradients.
+KINDS = (("graph", 1), ("eager", 0), ("sharded", 1))
+RUNS = [(kind, god, c) for kind, god in KINDS for cases in (CORE, SHAPES, SPLIT, LEAVES) for c in cases]
 
 
 def run_id(r):
-    env, god, cases = r
-    name = {id(CORE): "core", id(SHAPES): "shapes", id(SPLIT): "split", id(LEAVES): "leaves"}[id(cases)]
-    sw = "-".join("%s=%s" % (k[7:].lower(), v) for k, v in env.items()) or "defaults"
-    return "%s-%s-%s" % (name, sw, "devgrad" if god else "hostgrad")
+    kind, god, c = r
+    return "%s-%s-%s" % (kind, "devgrad" if god else "hostgrad", case_id(c))
 
 
 # ---------------------------------------------------------------------------------------------------------------- C ABI
@@ -265,12 +218,18 @@ def chk(lib, rc):
     assert rc == 0, lib.gpbdev_tree_last_error().decode()
 
 
-def create(lib, bins, num_bin, cfg):
+# the identity collective of a one-rank data-parallel learner (module level: the callback must outlive every learner using it)
+NOOP_ALLREDUCE = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_double), C.c_int64, C.c_void_p)(lambda ctx, buf, count, stream: 0)
+
+
+def create(lib, bins, num_bin, cfg, sharded=False):
     F, n = bins.shape
     h = C.c_void_p()
     nb = np.ascontiguousarray(num_bin, dtype=np.int32)
     chk(lib, lib.gpbdev_tree_create(C.byref(h), 0, C.c_int64(n), F, P(np.ascontiguousarray(bins), C.c_uint8), P(nb, C.c_int32),
                                     C.byref(cfg)))
+    if sharded:
+        chk(lib, lib.gpbdev_tree_set_allreduce(h, NOOP_ALLREDUCE, None, C.c_int64(n)))
     return h
 
 
@@ -326,17 +285,10 @@ def check_tree(d, a, exact, what=""):
         assert np.all(np.abs(d["split_gain"] - a["split_gain"]) <= np.spacing(np.abs(a["split_gain"]))), (what, "split_gain")
 
 
-def set_switches(monkeypatch, env):
-    for k in SWITCHES:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-
-
-def run_case(lib, c, on_device):
+def run_case(lib, c, on_device, sharded):
     bins, num_bin, grad, cfg, hess, want = case_data(c)
     n = bins.shape[1]
-    h = create(lib, bins, num_bin, cfg)
+    h = create(lib, bins, num_bin, cfg, sharded)
     g = None
     try:
         if on_device:
@@ -352,34 +304,41 @@ def run_case(lib, c, on_device):
 # ---------------------------------------------------------------------------------------------------------------- B
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", RUNS, ids=[run_id(r) for r in RUNS])
-def test_tree_matches_oracle(lib, run, monkeypatch):
-    env, on_device, cases = run
-    set_switches(monkeypatch, env)
-    for c in cases:
-        run_case(lib, c, on_device)
+def test_tree_matches_oracle(lib, run):
+    kind, on_device, c = run
+    run_case(lib, c, on_device, kind == "sharded")
 
 
 # ---------------------------------------------------------------------------------------------------------------- C
-def boost_data():
-    bins, num_bin = make_bins(4097, 33, 11)
+def boost_data(n, L, min_data, max_bin):
+    bins, num_bin = make_bins(n, 33, 11)
+    if max_bin:
+        num_bin = np.minimum(num_bin, max_bin).astype(np.int32)
+        bins = (bins % num_bin[:, None]).astype(np.uint8)
     label = (make_grad("cont", bins, num_bin, 11) + 3.).astype(np.float32)
-    return bins, num_bin, label, ot.make_config(num_leaves=31, min_data_in_leaf=5)
+    return bins, num_bin, label, ot.make_config(num_leaves=L, min_data_in_leaf=min_data)
+
+
+# (num_leaves, rows, min_data_in_leaf, bins per feature at most, sharded): 31 leaves = the graph, 300 = eager batches, and the
+# data-parallel sequence. Boosting gradients are continuous, and in a big tree many leaves leave bins empty: larger = parent - smaller
+# then holds a rounding residual instead of 0 there, which decides between thresholds of equal partition by noise (see make_grad).
+# At 300 leaves, leaves of >= 50 rows on <= 8 bins per feature keep every bin occupied.
+BOOST = [(31, 4097, 5, 0, False), (300, 100000, 50, 8, False), (31, 4097, 5, 0, True)]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("loop", ["host", "device", "graph"])
-def test_boosting_rounds_on_one_learner(lib, loop, monkeypatch):
+@pytest.mark.parametrize("L,n,min_data,max_bin,sharded", BOOST, ids=["L31", "L300", "L31-sharded"])
+def test_boosting_rounds_on_one_learner(lib, L, n, min_data, max_bin, sharded):
     """Five rounds of L2 boosting on ONE learner (ot.boost_l2 at kernel level): the gradient score - label is formed on the
     device into one fixed buffer, every tree grows from it, the shrunk leaf values are added to the device score. State carried
-    from tree to tree (histogram slots, splittable flags, the row-index buffers; on the graph loop the graph captured by the first
+    from tree to tree (histogram slots, splittable flags, the row-index buffers; on the graph the graph captured by the first
     tree and replayed by the others) must give the oracle's trees. Then a second gradient buffer and a new hessian constant,
     each of which must re-capture the graph, and the first buffer once more."""
-    set_switches(monkeypatch, {"GPB200_TREE_LOOP": loop})
-    bins, num_bin, label, cfg = boost_data()
+    bins, num_bin, label, cfg = boost_data(n, L, min_data, max_bin)
     n, lr = bins.shape[1], 0.1
     trees, score_o, init = ot.boost_l2(bins, num_bin, label, cfg, lr, 5)
     assert len(trees) == 5
-    h = create(lib, bins, num_bin, cfg)
+    h = create(lib, bins, num_bin, cfg, sharded)
     bufs = []
     try:
         score = dev_vec(lib, h, np.full(n, init)); lab = dev_vec(lib, h, label.astype(np.float64)); grad = dev_vec(lib, h, np.zeros(n))
@@ -405,18 +364,21 @@ def test_boosting_rounds_on_one_learner(lib, loop, monkeypatch):
         lib.gpbdev_tree_free(h)
 
 
+# (num_leaves, rows, min_data_in_leaf, gradient on the device): the graph, and the eager batches from host gradients
+LOOPS = [(31, 4097, 5, True), (300, 100000, 50, False)]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("loop", ["host", "graph"])
-def test_device_bins_constructor_matches_host_constructor(lib, loop, monkeypatch):
+@pytest.mark.parametrize("L,n,min_data,on_device", LOOPS, ids=["L31", "L300"])
+def test_device_bins_constructor_matches_host_constructor(lib, L, n, min_data, on_device):
     """The Booster's learner reads the bin matrix gpbdev_bin_matrix wrote (gpbdev_tree_create_on_device_bins); the kernel-level
     one transposes host bins itself (gpbdev_tree_create). Integer-valued columns with bin upper bounds k + 0.5 give the same bins,
     and both learners must grow the same tree, row for row."""
-    set_switches(monkeypatch, {"GPB200_TREE_LOOP": loop})
-    n, F = 4097, 40
+    F = 40
     Fpad = (F + 31) // 32 * 32
     bins, num_bin = make_bins(n, F, 21)
     grad = make_grad("cont", bins, num_bin, 21)
-    cfg = ot.make_config(num_leaves=31, min_data_in_leaf=5)
+    cfg = ot.make_config(num_leaves=L, min_data_in_leaf=min_data)
     X = np.ascontiguousarray(bins.T, dtype=np.float64)
     ub = np.full((F, 256), np.inf)
     for f in range(F):
@@ -436,6 +398,9 @@ def test_device_bins_constructor_matches_host_constructor(lib, loop, monkeypatch
                                                        C.byref(cfg)))
         h_host = create(lib, bins, num_bin, cfg)
         for h in (h_dev, h_host):
+            if not on_device:
+                trees.append(train(lib, h, n, cfg.num_leaves, grad, False))
+                continue
             g = dev_vec(lib, h, grad)
             try:
                 trees.append(train(lib, h, n, cfg.num_leaves, g, True))
@@ -447,7 +412,7 @@ def test_device_bins_constructor_matches_host_constructor(lib, loop, monkeypatch
             lib.gpbdev_tree_free(h_host)
         lib.gpbdev_bin_free(0, bins_dev)
     want = ot.train_tree(bins, num_bin, grad, cfg)
-    assert want["num_leaves"] == 31
+    assert want["num_leaves"] == L
     for k in trees[0]:
         assert np.array_equal(trees[0][k], trees[1][k]), k
     check_tree(trees[0], want, False)
@@ -474,24 +439,25 @@ def full_size():
     grad = rng.standard_normal(n)
     for f in range(12):
         grad += (bins[f] > 40 + 15 * f) * (0.3 if f % 2 else -0.25)
-    cfg = ot.make_config(num_leaves=31, min_data_in_leaf=20)
-    return bins, num_bin, grad, cfg, ot.train_tree(bins, num_bin, grad, cfg)
+    return bins, num_bin, grad
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("loop", ["host", "graph"])
-def test_full_size_tree_matches_oracle(lib, full_size, loop, monkeypatch):
-    """n = 1e6 x 50 features x 255 bins, 31 leaves: deep leaves still span several partition segments (max_seg = 4 x SMs of
-    >= 1024 rows) and several histogram chunks"""
-    set_switches(monkeypatch, {"GPB200_TREE_LOOP": loop})
-    bins, num_bin, grad, cfg, want = full_size
-    assert want["num_leaves"] == 31
+@pytest.mark.parametrize("L,on_device", [(31, True), (300, False)], ids=["L31", "L300"])
+def test_full_size_tree_matches_oracle(lib, full_size, L, on_device):
+    """n = 1e6 x 50 features x 255 bins: deep leaves still span several partition segments (max_seg = 4 x SMs of >= 1024 rows)
+    and several histogram chunks; 31 leaves on the graph, 300 eagerly from host gradients"""
+    bins, num_bin, grad = full_size
+    cfg = ot.make_config(num_leaves=L, min_data_in_leaf=20)
+    want = ot.train_tree(bins, num_bin, grad, cfg)
+    assert want["num_leaves"] == L
     n = bins.shape[1]
     h = create(lib, bins, num_bin, cfg)
     g = None
     try:
-        g = dev_vec(lib, h, grad)
-        got = train(lib, h, n, cfg.num_leaves, g, True)
+        if on_device:
+            g = dev_vec(lib, h, grad)
+        got = train(lib, h, n, cfg.num_leaves, g if on_device else grad, on_device)
     finally:
         if g is not None:
             lib.gpbdev_vec_free(h, g)
@@ -501,23 +467,26 @@ def test_full_size_tree_matches_oracle(lib, full_size, loop, monkeypatch):
 
 # ---------------------------------------------------------------------------------------------------------------- no GPU
 def test_cases_reach_every_kernel_path():
-    """Every combination of loop, histogram kernel, scan, advance and partition is run, so trimming RUNS cannot silently drop
-    one; the split knobs and gradient kinds run on all three scan implementations and on both loops with device state."""
-    reached = {path(env, c[2], god) for env, god, cases in RUNS for c in cases}
-    assert HOST_BUCKETS | DEVICE_BUCKETS <= reached
-    knob_paths = {path(env, c[2], god) for env, god, cases in RUNS if cases is SPLIT for c in cases}
-    assert {p[2] for p in knob_paths} == {"split_scan", "reduce_scan", "reduce_scan2"}
-    assert {p[0] for p in knob_paths} == {"host", "device", "graph"}
-    # the budgets cross the device-state boundary on the default switches
-    assert {path({}, L, 1)[0] for L in (256, 257)} == {"graph", "host"}
+    """Every path is run with one batch of splits and with several (the graph holds one batch by construction), so trimming RUNS
+    cannot silently drop one; every case set runs on every path; a tree that stops early stops in a later batch."""
+    reached = {(p, min(b, 2)) for p, b in (path(kind, c[2], god) for kind, god, c in RUNS)}
+    assert reached == {("graph", 1), ("eager", 1), ("eager", 2), ("sharded", 1), ("sharded", 2)}
+    for cases in (CORE, SHAPES, SPLIT, LEAVES):
+        assert {path(kind, c[2], god)[0] for kind, god, c in RUNS if c in cases} == {"graph", "eager", "sharded"}
+    assert {path("graph", L, 1)[0] for L in (256, 257)} == {"graph", "eager"}
     assert {c[0] for c in CORE + SHAPES} >= {2, 7, 9, 50, 257, 4097, 30000}
     assert {c[1] for c in CORE + SHAPES} >= {1, 4, 31, 32, 33, 64, 65, 96, 129, 200}
-    assert {c[2] for c in LEAVES} == {2, 3, 31, 255, 256, 257, 300}
+    assert {c[2] for c in LEAVES} == set(FILLED) | {EARLY_STOP}
+    early = [c for c in LEAVES if c[2] == EARLY_STOP]
+    assert len(early) == 1
+    grown = case_data(early[0])[5]["num_leaves"]
+    assert SPLIT_BATCH + 1 < grown < EARLY_STOP - SPLIT_BATCH, grown  # stops inside a batch after the first, before the last
 
 
 def test_leaf_budget_cases_fill_their_budget():
     for c in LEAVES:
-        assert case_data(c)[5]["num_leaves"] == c[2], case_id(c)
+        if c[2] in FILLED:
+            assert case_data(c)[5]["num_leaves"] == c[2], case_id(c)
 
 
 def test_knob_cases_bind():
