@@ -125,7 +125,7 @@ class GPModel(object):
                 if k in ("optimizer_cov", "init_cov_pars", "maxit", "delta_rel_conv", "lr_cov", "trace",
                          "convergence_criterion", "m_lbfgs", "estimate_cov_par_index", "std_dev", "cg_max_num_it",
                          "cg_max_num_it_tridiag", "cg_delta_conv", "num_rand_vec_trace", "seed_rand_vec_trace",
-                         "cg_preconditioner_type", "delta_conv_mode_finding", "optimizer_coef",
+                         "cg_preconditioner_type", "delta_conv_mode_finding", "optimizer_coef", "reuse_rand_vec_trace",
                          "init_coef_aux_pars_from_iid_model"):
                     self.params[k] = v
                 elif k == "init_coef":
@@ -220,12 +220,27 @@ class GPModel(object):
         return negll.value
 
     def get_cov_pars(self, std_err=False, format_pandas=False):
-        out = np.zeros(self.num_cov_pars, dtype=np.float64)
-        self._safe_call(self._LIB.GPB_GetCovPar(self.handle, _dptr(out), ctypes.c_bool(False)))
+        """Covariance parameters on the original scale (GPModel.get_cov_pars, basic.py:5964-6008). With `std_err` and a model
+        for which the library computes them, a 2 x num_cov_pars array: the parameters ("Param.") and their standard errors
+        ("Std. err."); otherwise the parameters alone."""
+        if std_err and not self._can_calculate_standard_errors_cov_pars():
+            std_err = False
+        k = self.num_cov_pars
+        out = np.zeros(2 * k if std_err else k, dtype=np.float64)
+        self._safe_call(self._LIB.GPB_GetCovPar(self.handle, _dptr(out), ctypes.c_bool(std_err)))
+        if std_err:
+            out = np.vstack((out[:k], out[k:]))
         if format_pandas:
             import pandas as pd
+            if std_err:
+                return pd.DataFrame(out, columns=self.cov_par_names, index=["Param.", "Std. err."])
             return pd.DataFrame(out.reshape(1, -1), columns=self.cov_par_names, index=["Param."])
         return out
+
+    def _can_calculate_standard_errors_cov_pars(self):
+        out = ctypes.c_int(0)
+        self._safe_call(self._LIB.GPB_CanCalculateStandardErrorsCovPars(self.handle, ctypes.byref(out)))
+        return bool(out.value)
 
     def laplace_info(self):
         """gpboost_b200 extension: (negll, Newton its, CG its, SLQ its, log det(Sigma W + I), objective at the mode)."""

@@ -118,6 +118,7 @@ FactorKernel pick_mode(int mode, int d, int m) {
     case gpb::MODE_NLL: return pick_dim<COV, gpb::MODE_NLL>(d, m);
     case gpb::MODE_STORE: return pick_dim<COV, gpb::MODE_STORE>(d, m);
     case gpb::MODE_GRAD: return pick_dim<COV, gpb::MODE_GRAD>(d, m);
+    case gpb::MODE_STORE_GRAD2: return pick_dim<COV, gpb::MODE_STORE_GRAD2>(d, m);
     default: return pick_dim<COV, gpb::MODE_STORE_GRAD>(d, m);
   }
 }
@@ -784,3 +785,4 @@ int gpbdev_vecchia_flush_l2(gpbdev_vecchia_t h) {
 #include "newton.cuh"
 #include "covariates.cuh"
 #include "laplace.cuh"
+#include "fisher.cuh"

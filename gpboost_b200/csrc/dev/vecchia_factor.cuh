@@ -42,7 +42,10 @@ enum CovType : int { COV_EXPONENTIAL = 0, COV_MATERN15 = 1, COV_MATERN25 = 2, CO
 // MODE_STORE_GRAD: MODE_STORE plus the derivative of the factor w.r.t. log(range): dA_i (= -B_grad row) and dD_i, what
 // CalcCovFactorGradientVecchia leaves in B_grad[1], D_grad[1] (Vecchia_utils.cpp:1636-1652) — needed where the derivative of
 // Sigma^-1 is applied to many vectors (Laplace-approximated likelihoods, likelihoods.h:6615-6690).
-enum FactorMode : int { MODE_NLL = 0, MODE_STORE = 1, MODE_GRAD = 2, MODE_STORE_GRAD = 3 };
+// MODE_STORE_GRAD2: the Gaussian (nugget) model's MODE_STORE plus the derivatives of the factor w.r.t. log(var) AND log(range)
+// on the transformed scale, what CalcCovFactorGradientVecchia leaves in B_grad[0..1], D_grad[0..1] — the Fisher information of
+// the covariance parameters (re_model_template.h:10145-10230) applies them to a block of probe vectors.
+enum FactorMode : int { MODE_NLL = 0, MODE_STORE = 1, MODE_GRAD = 2, MODE_STORE_GRAD = 3, MODE_STORE_GRAD2 = 4 };
 
 #ifndef GPB_NLL_BLOCKS
 #define GPB_NLL_BLOCKS 5
@@ -82,6 +85,9 @@ struct FactorArgs {
 // set with cudaMemcpyToSymbolAsync on the engine's stream right before the launch (one engine per device at a time).
 __device__ double* g_factor_dA = nullptr;
 __device__ double* g_factor_dD = nullptr;
+// MODE_STORE_GRAD2 only: d A_i / d log(var) (n x m) and d D_i / d log(var) (n); the range pair goes to g_factor_dA / g_factor_dD
+__device__ double* g_factor_dA0 = nullptr;
+__device__ double* g_factor_dD0 = nullptr;
 
 // exp(ax) for ax <= 0 (clamped at -700): round-to-nearest range reduction by the 1.5*2^52 trick, degree-13 Taylor
 // polynomial on |r| <= ln2/2 (truncation error 4e-18), scaling by an exponent-field add. No special-case paths and the
@@ -145,10 +151,12 @@ __device__ __forceinline__ double warp_sum(double x) {
 }
 
 template <int COV, int MODE, int DIM, int MT>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32, (MODE == MODE_GRAD || MODE == MODE_STORE_GRAD) ? GPB_GRAD_BLOCKS : GPB_NLL_BLOCKS)
+__global__ void __launch_bounds__(kWarpsPerBlock * 32,
+                                  (MODE == MODE_GRAD || MODE == MODE_STORE_GRAD || MODE == MODE_STORE_GRAD2) ? GPB_GRAD_BLOCKS : GPB_NLL_BLOCKS)
 vecchia_factor_kernel(const FactorArgs p) {
   constexpr bool GRAD = (MODE == MODE_GRAD);
-  constexpr bool GPAIR = GRAD || (MODE == MODE_STORE_GRAD);  // the range-derivative pair values are kept
+  constexpr bool DSTORE = (MODE == MODE_STORE_GRAD) || (MODE == MODE_STORE_GRAD2);  // the range derivative is stored
+  constexpr bool GPAIR = GRAD || DSTORE;  // the range-derivative pair values are kept
   constexpr bool SOLVE = (MODE != MODE_NLL);
   constexpr int P = MT + 1;      // point slots: 0..MT-1 neighbours (real or dummy), MT = the observation
   constexpr int NT = MT / 2;     // circulant rounds (P is odd)
@@ -332,11 +340,11 @@ vecchia_factor_kernel(const FactorArgs p) {
       // xa = A_i[lane] for lane < q
       const double Dinv_i = 1. / Di;
       const double By = r_over_sd * sqrt(Di);
-      if (MODE == MODE_STORE || MODE == MODE_STORE_GRAD) {
+      if (MODE == MODE_STORE || DSTORE) {
         if (lane < m) p.A[i * m + lane] = (lane < q) ? xa : 0.;
         if (lane == 0) { p.Dinv[i] = Dinv_i; p.w[i] = By * Dinv_i; }
       }
-      if (MODE == MODE_STORE_GRAD) {
+      if (DSTORE) {
         // r = dSigma~ b over the P points (b = [-A, 1]): rows 0..MT-1 of r are dSigma_iN - dSigma_NN A, and b.r = dD
         __syncwarp();
         xb[lane] = (lane < MT) ? -xa : (lane == MT ? 1. : 0.);
@@ -375,6 +383,28 @@ vecchia_factor_kernel(const FactorArgs p) {
         }
         if (lane < m) g_factor_dA[i * m + lane] = (lane < q) ? xg : 0.;
         if (lane == 0) g_factor_dD[i] = dDv;
+      }
+      if (MODE == MODE_STORE_GRAD2) {
+        // log(var): dSigma~ = Sigma~ - I (the nugget does not move), so dA = S^-1 (s - (S - I) A) = S^-1 A and
+        // dD = var - dA.s - A.s = D - 1 - A.A  (A.s = 1 + var - D; Vecchia_utils.cpp:1571, :1623, :1636-1652)
+        double xv = (lane < MT) ? xa : 0.;
+#pragma unroll
+        for (int j = 0; j < MT; ++j) {
+          const double wj = shfl_d(xv * dinv, j);
+          const double lij = (lane > j && lane < MT) ? S[j * kLd + lane] : 0.;
+          if (lane == j) xv = wj;
+          xv -= lij * wj;
+        }
+#pragma unroll
+        for (int r = MT - 1; r >= 0; --r) {
+          const double fa = shfl_d(xv * dinv, r);
+          const double lrc = (lane < r) ? S[lane * kLd + r] : 0.;
+          if (lane == r) xv = fa;
+          xv -= lrc * fa;
+        }
+        const double aa = warp_sum((lane < q) ? xa * xa : 0.);
+        if (lane < m) g_factor_dA0[i * m + lane] = (lane < q) ? xv : 0.;
+        if (lane == 0) g_factor_dD0[i] = Di - 1. - aa;
       }
       if (GRAD) {
         // b = [-A, 1], w~ = [w, 0] over the P points

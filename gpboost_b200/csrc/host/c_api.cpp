@@ -51,6 +51,13 @@ const char* LGBM_GetLastError(void) { return g_last_error; }
 // reference's Log:: is not part of the hot path), the callback is kept for messages raised through it
 static void (*g_log_callback)(const char*) = nullptr;
 int LGBM_RegisterLogCallback(void (*callback)(const char*)) { g_log_callback = callback; return 0; }
+}  // extern "C"
+
+void gpb200::LogWarning(const char* msg) {
+  if (g_log_callback != nullptr) g_log_callback((std::string("[GPBoost] [Warning] ") + msg + "\n").c_str());
+}
+
+extern "C" {
 __attribute__((visibility("default"))) void GPB200_SetLastErrorMessage(const char* msg) { SetLastError(msg); }  // for c_api_scope.cpp
 
 int GPB_CreateREModel(int32_t num_data, const int32_t* cluster_ids_data, const char* re_group_data, int32_t num_re_group,
@@ -85,14 +92,14 @@ int GPB_SetOptimConfig(REModelHandle handle, double* init_cov_pars, double lr, d
                        const char* optimizer, int /*momentum_offset*/, const char* convergence_criterion,
                        int num_covariates, double* init_coef, double /*lr_coef*/, double /*acc_rate_coef*/,
                        const char* optimizer_coef, int cg_max_num_it, int cg_max_num_it_tridiag,
-                       double cg_delta_conv, int num_rand_vec_trace, bool /*reuse_rand_vec_trace*/,
+                       double cg_delta_conv, int num_rand_vec_trace, bool reuse_rand_vec_trace,
                        const char* cg_preconditioner_type, int seed_rand_vec_trace, int /*piv_chol_rank*/,
                        double* /*init_aux_pars*/, bool /*estimate_aux_pars*/, bool init_coef_aux_pars_from_iid_model,
                        const int* estimate_cov_par_index, int m_lbfgs, double delta_conv_mode_finding) {
   API_BEGIN();
   M(handle)->SetCoefOptimConfig(num_covariates, init_coef, optimizer_coef, init_coef_aux_pars_from_iid_model);
   M(handle)->SetIterativeConfig(cg_max_num_it, cg_max_num_it_tridiag, cg_delta_conv, num_rand_vec_trace, cg_preconditioner_type,
-                                seed_rand_vec_trace, delta_conv_mode_finding);
+                                seed_rand_vec_trace, delta_conv_mode_finding, reuse_rand_vec_trace);
   M(handle)->SetOptimConfig(init_cov_pars, lr, max_iter, delta_rel_conv, trace, optimizer, convergence_criterion, m_lbfgs,
                             estimate_cov_par_index);
   API_END();
@@ -217,10 +224,10 @@ int GPB_PredictREModel(REModelHandle handle, const double* y_data, int32_t num_d
   API_END();
 }
 
+// 1 exactly when GPB_GetCovPar(..., calc_std_dev = true) computes them (REModel::CanCalculateStandardErrorsCovPars)
 int GPB_CanCalculateStandardErrorsCovPars(REModelHandle handle, int* out) {
   API_BEGIN();
-  M(handle);
-  *out = 0;
+  *out = M(handle)->StdDevCovParsUnsupportedReason().empty() ? 1 : 0;
   API_END();
 }
 

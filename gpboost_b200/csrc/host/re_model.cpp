@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <numeric>
 #include <stdexcept>
 #include <unordered_map>
@@ -404,8 +405,10 @@ double REModel::TransformRange(double range) const {
 }
 
 void REModel::SetIterativeConfig(int cg_max_num_it, int cg_max_num_it_tridiag, double cg_delta_conv, int num_rand_vec_trace,
-                                 const char* cg_preconditioner_type, int seed_rand_vec_trace, double delta_conv_mode_finding) {
+                                 const char* cg_preconditioner_type, int seed_rand_vec_trace, double delta_conv_mode_finding,
+                                 bool reuse_rand_vec_trace) {
   // re_model_template.h:860-900: non-positive / -999 values keep the defaults
+  reuse_rand_vec_trace_ = reuse_rand_vec_trace;
   if (cg_max_num_it > 0) cg_max_num_it_ = cg_max_num_it;
   if (cg_max_num_it_tridiag > 0) cg_max_num_it_tridiag_ = cg_max_num_it_tridiag;
   if (cg_delta_conv > 0.) cg_delta_conv_ = cg_delta_conv;
@@ -423,6 +426,18 @@ void REModel::SetIterativeConfig(int cg_max_num_it, int cg_max_num_it_tridiag, d
 // GenRandVecNormalParallel (src/GPBoost/CG_utils.cpp:978-994): column col_i of the probe matrix is drawn from
 // mt19937(seed_seq{seed, run_id lo, run_id hi, col_i}) with std::normal_distribution — the same standard-library calls,
 // so the stochastic Lanczos quadrature sees the reference's probe vectors. Rows index the latent process in Vecchia order.
+static void DrawProbes(int seed, uint64_t run_id, int32_t n, const std::vector<int>& cols, double* out) {
+  const uint32_t b32 = static_cast<uint32_t>(seed);
+#pragma omp parallel for schedule(static) num_threads(16)
+  for (int lc = 0; lc < (int)cols.size(); ++lc) {
+    std::normal_distribution<double> ndist(0.0, 1.0);
+    std::seed_seq seq{b32, static_cast<uint32_t>(run_id), static_cast<uint32_t>(run_id >> 32), static_cast<uint32_t>(cols[lc])};
+    std::mt19937 gen(seq);
+    double* dst = out + (size_t)lc * n;
+    for (int32_t row = 0; row < n; ++row) dst[row] = ndist(gen);
+  }
+}
+
 void REModel::EnsureProbes() {
   if (probes_t_ == num_rand_vec_trace_ && probes_seed_ == seed_rand_vec_trace_) return;  // reuse_rand_vec_trace
   const int t = num_rand_vec_trace_;
@@ -433,16 +448,7 @@ void REModel::EnsureProbes() {
   if (cols.empty()) Fatal("num_rand_vec_trace is smaller than the number of ranks");
   const int tl = (int)cols.size();
   std::vector<double> probes((size_t)num_data_ * tl);
-  const uint64_t run_id = cg_generator_counter_;
-  const uint32_t b32 = static_cast<uint32_t>(seed_rand_vec_trace_);
-#pragma omp parallel for schedule(static) num_threads(16)
-  for (int lc = 0; lc < tl; ++lc) {
-    std::normal_distribution<double> ndist(0.0, 1.0);
-    std::seed_seq seq{b32, static_cast<uint32_t>(run_id), static_cast<uint32_t>(run_id >> 32), static_cast<uint32_t>(cols[lc])};
-    std::mt19937 gen(seq);
-    double* dst = probes.data() + (size_t)lc * num_data_;
-    for (int32_t row = 0; row < num_data_; ++row) dst[row] = ndist(gen);
-  }
+  DrawProbes(seed_rand_vec_trace_, cg_generator_counter_, num_data_, cols, probes.data());
   ++cg_generator_counter_;
   DevCheck(gpbdev_vecchia_laplace_set_probes(engine_, probes.data(), tl));
   if (rt.world_size > 1) {
@@ -657,6 +663,7 @@ void REModel::Predict(const double* y_obs, int32_t num_data_pred, double* out_pr
 
 void REModel::OptimCovPar(const double* y_data, const double* fixed_effects, bool called_in_GPBoost_algorithm,
                           bool reuse_learning_rates_from_previous_call) {
+  std_dev_cov_pars_calculated_ = false;  // re_model.cpp:543, :629
   if (!gauss_) {
     // L-BFGS on log(cov_pars) with the device gradient of the Laplace-approximated likelihood (tests/test_laplace_gpu.py: gradient and
     // fits against the reference's goldens on the GPU; tests/test_laplace_oracle_pinned.py: the same driver fed by the oracle)
@@ -749,6 +756,7 @@ void REModel::SetYDevice(const double* y_dev) {
 }
 
 void REModel::OptimCovParDevice(const double* y_dev, bool called_in_GPBoost_algorithm, bool reuse_learning_rates_from_previous_call) {
+  std_dev_cov_pars_calculated_ = false;  // re_model.cpp:543, :629
   if (y_dev == nullptr) Fatal("Check failed: y_data != nullptr");
   if (!DevicePathReady()) Fatal("OptimCovParDevice: no device-resident path for this model state (use OptimCovPar)");
   num_covariates_ = 0;
@@ -999,6 +1007,7 @@ void REModel::ProfileOutCoef(double var, double range) {
 }
 
 void REModel::OptimLinRegrCoefCovPar(const double* y_data, const double* covariate_data, int num_covariates, const double* fixed_effects) {
+  std_dev_cov_pars_calculated_ = false;  // re_model.cpp:543, :629
   if (covariate_data == nullptr || num_covariates <= 0) {  // no covariates: the same optimisation as GPB_OptimCovPar
     OptimCovPar(y_data, fixed_effects, false, false);
     return;
@@ -1086,10 +1095,85 @@ void REModel::GetCovariateData(double* out) const {
   std::copy(X_.begin(), X_.end(), out);
 }
 
-void REModel::GetCovPar(double* out, bool calc_std_dev) const {
+void REModel::GetCovPar(double* out, bool calc_std_dev) {
   if (!cov_pars_initialized_) Fatal("Covariance parameters have not been estimated or set");
-  if (calc_std_dev) Fatal("Standard deviations of covariance parameters are not available in the CUDA engine");
+  if (calc_std_dev) {
+    const std::string why = StdDevCovParsUnsupportedReason();
+    if (!why.empty()) Fatal(why);
+  }
   TransformBackCovPars(cov_pars_.data(), out);
+  if (!calc_std_dev) return;
+  if (!std_dev_cov_pars_calculated_) {
+    CalcStdDevCovPar();
+    std_dev_cov_pars_calculated_ = true;
+  }
+  std::copy(std_dev_cov_pars_.begin(), std_dev_cov_pars_.end(), out + num_cov_pars_);
+}
+
+std::string REModel::StdDevCovParsUnsupportedReason() const {
+  const std::string pre = "Standard errors of covariance parameters are not available in the CUDA engine ";
+  if (!gauss_) return pre + "for likelihood '" + likelihood_ + "' (only for 'gaussian')";
+  if (engine_ == nullptr) return pre + "for this model (only for a Gaussian process with gp_approx = 'vecchia')";
+  const Runtime& rt = GetRuntime();
+  if (rt.world_size > 1) return pre + "for a model whose observations are sharded over several GPUs";
+  if (num_neighbors_ > 30) return pre + "for num_neighbors > 30 (found " + std::to_string(num_neighbors_) + ")";
+  return "";
+}
+
+// CalcStdDevCovPar (re_model_template.h:10788-10815): Fisher information on the original scale by the stochastic trace estimator
+// (CalcFisherInformation_Vecchia, :10145-10230), std_dev = sqrt(diag(FI^-1)) through a Cholesky factor; NaN entries and a warning
+// when FI is not positive definite. The probe vectors are drawn as the reference draws rand_vec_fisher_info_: once per model with
+// reuse_rand_vec_trace, otherwise anew for every computation, each draw advancing cg_generator_counter_.
+void REModel::CalcStdDevCovPar() {
+  if (!saved_rand_vec_fisher_info_) {
+    const int t = num_rand_vec_trace_;
+    std::vector<int> cols(t);
+    std::iota(cols.begin(), cols.end(), 0);
+    rand_vec_fisher_info_.resize((size_t)num_data_ * t);
+    DrawProbes(seed_rand_vec_trace_, cg_generator_counter_, num_data_, cols, rand_vec_fisher_info_.data());
+    ++cg_generator_counter_;
+    rand_vec_fisher_info_t_ = t;
+    if (reuse_rand_vec_trace_) saved_rand_vec_fisher_info_ = true;
+  }
+  double FI[9];
+  DevCheck(gpbdev_vecchia_fisher_info(engine_, cov_id_, cov_pars_[0], cov_pars_[1], cov_pars_[2], rand_vec_fisher_info_.data(),
+                                      rand_vec_fisher_info_t_, FI));
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  std_dev_cov_pars_.assign(3, nan);
+  // Eigen::LLT: fails on a non-positive (or NaN) pivot
+  double L[9] = {0., 0., 0., 0., 0., 0., 0., 0., 0.};
+  bool ok = true;
+  for (int j = 0; j < 3 && ok; ++j) {
+    double d = FI[j * 3 + j];
+    for (int k = 0; k < j; ++k) d -= L[j * 3 + k] * L[j * 3 + k];
+    if (!(d > 0.)) { ok = false; break; }
+    d = std::sqrt(d);
+    L[j * 3 + j] = d;
+    for (int i = j + 1; i < 3; ++i) {
+      double v = FI[i * 3 + j];
+      for (int k = 0; k < j; ++k) v -= L[i * 3 + k] * L[j * 3 + k];
+      L[i * 3 + j] = v / d;
+    }
+  }
+  if (!ok) {
+    LogWarning("Cannot calculate standard deviations for covariance parameters since the Fisher information is not positive definite ");
+    return;
+  }
+  for (int c = 0; c < 3; ++c) {  // column c of FI^-1 = L^-T L^-1 e_c; only its diagonal entry is kept
+    double x[3] = {0., 0., 0.};
+    x[c] = 1.;
+    for (int i = 0; i < 3; ++i) {
+      double v = x[i];
+      for (int k = 0; k < i; ++k) v -= L[i * 3 + k] * x[k];
+      x[i] = v / L[i * 3 + i];
+    }
+    for (int i = 2; i >= 0; --i) {
+      double v = x[i];
+      for (int k = i + 1; k < 3; ++k) v -= L[k * 3 + i] * x[k];
+      x[i] = v / L[i * 3 + i];
+    }
+    if (std::isfinite(x[c]) && x[c] >= 0.) std_dev_cov_pars_[c] = std::sqrt(x[c]);
+  }
 }
 
 void REModel::GetInitCovPar(double* out) const {

@@ -51,7 +51,8 @@ class REModel {
   void GetCovariateData(double* out) const;
   int NumCovariates() const { return num_covariates_; }
   void SetIterativeConfig(int cg_max_num_it, int cg_max_num_it_tridiag, double cg_delta_conv, int num_rand_vec_trace,
-                          const char* cg_preconditioner_type, int seed_rand_vec_trace, double delta_conv_mode_finding);
+                          const char* cg_preconditioner_type, int seed_rand_vec_trace, double delta_conv_mode_finding,
+                          bool reuse_rand_vec_trace = true);
   // REModel::OptimCovPar (re_model.cpp:483-541)
   void OptimCovPar(const double* y_data, const double* fixed_effects, bool called_in_GPBoost_algorithm,
                    bool reuse_learning_rates_from_previous_call);
@@ -79,8 +80,11 @@ class REModel {
   void Predict(const double* y_obs, int32_t num_data_pred, double* out_predict, bool predict_cov_mat, bool predict_var,
                bool predict_response, const double* gp_coords_data_pred, const double* cov_pars_pred, bool use_saved_data,
                const double* fixed_effects, const double* covariate_data_pred = nullptr);
-  // GPB_GetCovPar / GPB_GetInitCovPar (original scale)
-  void GetCovPar(double* out, bool calc_std_dev) const;
+  // GPB_GetCovPar / GPB_GetInitCovPar (original scale). With calc_std_dev the standard errors follow in out[num_cov_pars ..
+  // 2 num_cov_pars) (REModel::GetCovPar, re_model.cpp:921-965): computed once per fit and cached.
+  void GetCovPar(double* out, bool calc_std_dev);
+  // why GetCovPar(..., true) is refused for this model, or "" when it computes the standard errors
+  std::string StdDevCovParsUnsupportedReason() const;
   void GetInitCovPar(double* out) const;
   int GetNumIt() const { return num_it_; }
   int NumCovPars() const { return num_cov_pars_; }
@@ -137,6 +141,14 @@ class REModel {
   // checks poisson labels (non-negative integers) and returns -sum_i log(y_i!)
   double CheckCountsLogNormConst(const double* y) const;
   void EnsureProbes();
+  // CalcStdDevCovPar (re_model_template.h:10788-10815) for the Gaussian Vecchia model: std_dev_cov_pars_ from the device Fisher information
+  void CalcStdDevCovPar();
+  std::vector<double> std_dev_cov_pars_;
+  bool std_dev_cov_pars_calculated_ = false;  // cleared by every fit (re_model.cpp:543, :629)
+  bool reuse_rand_vec_trace_ = true;
+  std::vector<double> rand_vec_fisher_info_;  // n x t column-major, Vecchia order (re_model_template.h:10151-10156)
+  int rand_vec_fisher_info_t_ = 0;
+  bool saved_rand_vec_fisher_info_ = false;
   double TransformRange(double range) const;
   int cg_max_num_it_ = 1000, cg_max_num_it_tridiag_ = 1000, num_rand_vec_trace_ = 50, seed_rand_vec_trace_ = 1;
   double cg_delta_conv_ = 1e-2, delta_conv_mode_finding_ = 1e-8;

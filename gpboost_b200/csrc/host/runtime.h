@@ -19,5 +19,7 @@ struct Runtime {
   void* allreduce_ctx = nullptr;
 };
 Runtime& GetRuntime();
+// a warning through the log callback the bindings registered (LGBM_RegisterLogCallback), formatted like Log::REWarning
+void LogWarning(const char* msg);
 }  // namespace gpb200
 #endif

@@ -118,6 +118,16 @@ GPBDEV_EXPORT int gpbdev_vecchia_gls_residual(gpbdev_vecchia_t h, const double* 
  * Vecchia order; Dinv, dD: n). Diagnostics / test entry of the factor kernel's MODE_STORE_GRAD. */
 GPBDEV_EXPORT int gpbdev_vecchia_latent_factor_grad(gpbdev_vecchia_t h, int cov_type, double var, double range, double* A_host,
                                                     double* Dinv_host, double* dA_host, double* dD_host);
+/* Fisher information of the Gaussian Vecchia model's covariance parameters on the ORIGINAL scale, ordered (sigma2, sigma1^2, rho):
+ * CalcFisherInformation_Vecchia with the stochastic trace estimator, transf_scale = false, include_error_var = true
+ * (include/GPBoost/re_model_template.h:10145-10230), at the factor and derivatives of CalcStdDevCovPar (:10788-10815).
+ * sigma2 = error variance; var = sigma1^2 / sigma2 and range transformed as for gpbdev_vecchia_eval. probes_colmajor: host, n x t
+ * column-major, rows in the Vecchia order (GenRandVecNormalParallel, CG_utils.cpp:978-994), t >= 1; columns are processed in blocks
+ * of at most 128 and summed in column order (two calls give bitwise the same result). FI9: host, 3 x 3 row-major (symmetric).
+ * Whole-model engines with num_neighbors <= 30 only. The factor is formed in buffers of the call's own: the engine's stored factor,
+ * its last sums and its STORE shortcut state are not touched. */
+GPBDEV_EXPORT int gpbdev_vecchia_fisher_info(gpbdev_vecchia_t h, int cov_type, double sigma2, double var, double range,
+                                             const double* probes_colmajor, int t, double* FI9);
 /* After a STORE eval: copy A (n x m) and D^-1 (n) to the host — parity tests against the oracle's B, D^-1 */
 GPBDEV_EXPORT int gpbdev_vecchia_get_factor(gpbdev_vecchia_t h, double* A_host, double* Dinv_host);
 
