@@ -5,5 +5,6 @@
 """
 from .basic import GPModel, GPBoostError  # noqa: F401
 from .libpath import load_lib, find_lib_path  # noqa: F401
+from .engine import train  # noqa: F401
 
 __version__ = "0.1.0"

@@ -301,6 +301,42 @@ class GPModel(object):
             None, None, None, _dptr(Xp), None, cp_c, xp_c, ctypes.c_bool(True), None, None))
         return {"mu": out[:npred].copy(), "var": out[npred:].copy() if predict_var else None}
 
+    def set_prediction_data(self, gp_coords_pred=None, vecchia_pred_type=None, num_neighbors_pred=None, X_pred=None):
+        """Set the prediction data (GPModel.set_prediction_data, basic.py): the GP coordinates of the validation data the GPBoost
+        algorithm predicts at with `use_gp_model_for_validation=True`."""
+        if gp_coords_pred is None and X_pred is None and vecchia_pred_type is None and num_neighbors_pred is None:
+            raise ValueError("No prediction data given")
+        coords_c, npred = None, 0
+        if gp_coords_pred is not None:
+            gp_coords_pred = np.asarray(gp_coords_pred, dtype=np.float64)
+            if gp_coords_pred.ndim == 1:
+                gp_coords_pred = gp_coords_pred.reshape(-1, 1)
+            if gp_coords_pred.ndim != 2 or gp_coords_pred.shape[1] != self.dim_coords:
+                raise ValueError("Incorrect number of dimensions / columns in 'gp_coords_pred'")
+            npred = gp_coords_pred.shape[0]
+            self._coords_pred_c = np.asfortranarray(gp_coords_pred)
+            coords_c = _dptr(self._coords_pred_c)
+        xp_c = None
+        if X_pred is not None:
+            X_pred = np.asarray(X_pred, dtype=np.float64)
+            if X_pred.ndim == 1:
+                X_pred = X_pred.reshape(-1, 1)
+            if npred and X_pred.shape[0] != npred:
+                raise ValueError("Incorrect number of data points in 'X_pred'")
+            npred = X_pred.shape[0]
+            self._Xpred_saved_c = np.ascontiguousarray(X_pred.flatten(order="F"))
+            xp_c = _dptr(self._Xpred_saved_c)
+        self._safe_call(self._LIB.GPB_SetPredictionData(
+            self.handle, ctypes.c_int32(npred), None, None, None, coords_c, None, xp_c,
+            c_str(vecchia_pred_type) if vecchia_pred_type else None,
+            ctypes.c_int(-1 if num_neighbors_pred is None else int(num_neighbors_pred)), ctypes.c_double(-1.),
+            ctypes.c_int(-1), ctypes.c_int(-1)))
+        if gp_coords_pred is not None:
+            self.prediction_data_is_set = True
+        return self
+
+    prediction_data_is_set = False
+
     # ---- CUDA-build extensions ------------------------------------------------------------------------
     def response_gradient(self, y):
         """Psi^-1 y / sigma^2 at the current covariance parameters (what the boosting objective consumes)."""

@@ -12,13 +12,23 @@ C_API_DTYPE_FLOAT32, C_API_DTYPE_FLOAT64 = 0, 1
 C_API_PREDICT_NORMAL, C_API_PREDICT_RAW_SCORE = 0, 1
 
 
+def _param_value_str(v):
+    if isinstance(v, bool):
+        return str(v).lower()
+    if isinstance(v, (list, tuple, set)):  # e.g. metric=["l2", "rmse"] -> "l2,rmse" (param_dict_to_str, basic.py)
+        return ",".join(str(x) for x in v)
+    return v
+
+
 def param_dict_to_str(params):
-    return " ".join("%s=%s" % (k, str(v).lower() if isinstance(v, bool) else v) for k, v in (params or {}).items())
+    return " ".join("%s=%s" % (k, _param_value_str(v)) for k, v in (params or {}).items())
 
 
 class Dataset(object):
-    def __init__(self, data, label=None, params=None, _lib=None):
+    def __init__(self, data, label=None, params=None, reference=None, _lib=None):
+        """`reference`: the training Dataset whose bin mappers bin this one (validation data, Dataset(..., reference=train_set))."""
         self._LIB = load_lib() if _lib is None else _lib
+        self.reference = reference
         data = np.asarray(data)
         # float32 matrices are passed as they are (C_API_DTYPE_FLOAT32), like the reference's package (basic.py: __init_from_np2d)
         dt = np.float32 if data.dtype == np.float32 else np.float64
@@ -29,7 +39,8 @@ class Dataset(object):
         self.handle = ctypes.c_void_p()
         self._safe_call(self._LIB.LGBM_DatasetCreateFromMat(
             data.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(C_API_DTYPE_FLOAT32 if dt == np.float32 else C_API_DTYPE_FLOAT64), ctypes.c_int32(self.num_data),
-            ctypes.c_int32(self.num_feature), ctypes.c_int(1), c_str(param_dict_to_str(params)), None, ctypes.byref(self.handle)))
+            ctypes.c_int32(self.num_feature), ctypes.c_int(1), c_str(param_dict_to_str(params)),
+            None if reference is None else reference.handle, ctypes.byref(self.handle)))
         if label is not None:
             self.set_label(label)
 
@@ -59,6 +70,10 @@ class Booster(object):
         self._LIB = load_lib() if _lib is None else _lib
         self.train_set, self.gp_model = train_set, gp_model
         self.handle = ctypes.c_void_p()
+        self.valid_sets, self.name_valid_sets = [], []
+        self._train_data_name = "training"
+        self.best_iteration = 0
+        self.__eval_names = None
         if model_str is not None or model_file is not None:  # prediction-only booster (Booster(model_file=...), basic.py:2404-2425)
             n_it = ctypes.c_int(0)
             if model_str is not None:
@@ -112,6 +127,69 @@ class Booster(object):
         self._safe_call(self._LIB.LGBM_BoosterGetNumPredict(self.handle, ctypes.c_int(0), ctypes.byref(n)))
         out = np.empty(n.value, dtype=np.float64)
         self._safe_call(self._LIB.LGBM_BoosterGetPredict(self.handle, ctypes.c_int(0), ctypes.byref(n), _dptr(out)))
+        return out
+
+    # ---- validation data and metrics (Booster.add_valid / eval_train / eval_valid, basic.py) ---------------------------------
+    def set_train_data_name(self, name):
+        self._train_data_name = name
+        return self
+
+    def add_valid(self, data, name):
+        """Add validation data: `data` is a Dataset built with `reference=` the training Dataset."""
+        if not isinstance(data, Dataset):
+            raise TypeError("Validation data should be Dataset instance, met {}".format(type(data).__name__))
+        if data.reference is not self.train_set:
+            raise GPBoostError("Add validation data failed, you should use same predictor for these data")
+        self._safe_call(self._LIB.LGBM_BoosterAddValidData(self.handle, data.handle))
+        self.valid_sets.append(data)
+        self.name_valid_sets.append(name)
+        return self
+
+    def _eval_names(self):
+        if self.__eval_names is None:
+            n = ctypes.c_int(0)
+            self._safe_call(self._LIB.LGBM_BoosterGetEvalCounts(self.handle, ctypes.byref(n)))
+            names = []
+            if n.value > 0:
+                buf_len = 255
+                bufs = [ctypes.create_string_buffer(buf_len) for _ in range(n.value)]
+                ptrs = (ctypes.c_char_p * n.value)(*map(ctypes.addressof, bufs))
+                out_len, req = ctypes.c_int(0), ctypes.c_size_t(0)
+                self._safe_call(self._LIB.LGBM_BoosterGetEvalNames(self.handle, ctypes.c_int(n.value), ctypes.byref(out_len),
+                                                                   ctypes.c_size_t(buf_len), ctypes.byref(req), ptrs))
+                names = [b.value.decode("utf-8") for b in bufs[:out_len.value]]
+            self.__eval_names = names
+        return self.__eval_names
+
+    def _inner_eval(self, data_name, data_idx):
+        names = self._eval_names()
+        if not names:
+            return []
+        out = np.zeros(len(names), dtype=np.float64)
+        n = ctypes.c_int(0)
+        self._safe_call(self._LIB.LGBM_BoosterGetEval(self.handle, ctypes.c_int(data_idx), ctypes.byref(n), _dptr(out)))
+        if n.value != len(names):
+            raise ValueError("Wrong length of eval results")
+        # every metric of this build (l2, rmse, l1, test_neg_log_likelihood) is better when lower
+        return [(data_name, names[i], float(out[i]), False) for i in range(len(names))]
+
+    def eval_train(self):
+        """Metrics on the training data: list of (data_name, eval_name, value, is_higher_better)."""
+        return self._inner_eval(self._train_data_name, 0)
+
+    def eval_valid(self):
+        """Metrics on every validation set, in the order they were added."""
+        out = []
+        for i, name in enumerate(self.name_valid_sets):
+            out.extend(self._inner_eval(name, i + 1))
+        return out
+
+    def inner_predict(self, data_idx):
+        """Raw scores of data set `data_idx` (0 training data, k the k-th validation set)."""
+        n = ctypes.c_int64(0)
+        self._safe_call(self._LIB.LGBM_BoosterGetNumPredict(self.handle, ctypes.c_int(data_idx), ctypes.byref(n)))
+        out = np.empty(n.value, dtype=np.float64)
+        self._safe_call(self._LIB.LGBM_BoosterGetPredict(self.handle, ctypes.c_int(data_idx), ctypes.byref(n), _dptr(out)))
         return out
 
     def predict(self, data, raw_score=True, start_iteration=0, num_iteration=-1):

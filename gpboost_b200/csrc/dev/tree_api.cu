@@ -596,6 +596,68 @@ __global__ void add_const_kernel(double* __restrict__ a, double c, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) a[i] += c;
 }
 
+// ---- validation data ----------------------------------------------------------------------------------------------------------
+// score[i] += leaf_value[leaf(i)] (Tree::AddPredictionToScore, tree.h:104-120): one thread per row walks the tree on the row's bins,
+// bin <= threshold_bin -> left (the bin form of NumericalDecision for bins made by the training data's bin mappers). Nodes are one
+// int4 each, read through the read-only cache; every row touches one byte per level of its own row.
+__global__ void __launch_bounds__(256) valid_tree_score_kernel(const uint8_t* __restrict__ bins, int Fpad, int64_t n,
+                                                               const int4* __restrict__ nodes, const double* __restrict__ leaf_value,
+                                                               double* __restrict__ score) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint8_t* __restrict__ row = bins + i * Fpad;
+    int node = 0;
+    while (node >= 0) {
+      const int4 nd = __ldg(nodes + node);
+      node = (int)row[nd.x] <= nd.y ? nd.z : nd.w;
+    }
+    score[i] += __ldg(leaf_value + ~node);
+  }
+}
+
+// Metric sums (RegressionMetric / TestNegLogLikelihood, regression_metric.hpp): kMetricAcc accumulators per row, fixed contiguous
+// block ranges and a fixed shared-memory tree, then one block per accumulator sums the block partials in block order.
+constexpr int kMetricAcc = 4;
+constexpr int kMetricMaxBlocks = 1024;
+__global__ void __launch_bounds__(256) metric_stage1_kernel(const double* __restrict__ score, const double* __restrict__ label, int64_t n,
+                                                            const double* __restrict__ gp_mean, const double* __restrict__ gp_dvar,
+                                                            double sigma2, double shift, double* __restrict__ part) {
+  __shared__ double sh[kMetricAcc][256];
+  double s_sq = 0., s_abs = 0., s_lin = 0., s_nll = 0.;
+  const int64_t per = (n + gridDim.x - 1) / gridDim.x;
+  const int64_t b = (int64_t)blockIdx.x * per, e = min(b + per, n);
+  for (int64_t i = b + threadIdx.x; i < e; i += blockDim.x) {
+    double p = score[i];
+    if (gp_mean) p -= gp_mean[i];  // score - (mean of F - y): the GP's prediction of y - F added to F (regression_metric.hpp:102)
+    const double r = p - label[i];
+    const double rs = r + shift;
+    s_sq += rs * rs;
+    s_abs += fabs(r);
+    s_lin += r;
+    if (gp_dvar) {
+      const double v = sigma2 * (gp_dvar[i] + 1.);  // response variance: sigma^2 D_p plus the nugget sigma^2 (REModel::Predict)
+      s_nll += r * r / v + log(v);
+    }
+  }
+  sh[0][threadIdx.x] = s_sq; sh[1][threadIdx.x] = s_abs; sh[2][threadIdx.x] = s_lin; sh[3][threadIdx.x] = s_nll;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o)
+      for (int k = 0; k < kMetricAcc; ++k) sh[k][threadIdx.x] += sh[k][threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x < kMetricAcc) part[(size_t)threadIdx.x * kMetricMaxBlocks + blockIdx.x] = sh[threadIdx.x][0];
+}
+__global__ void __launch_bounds__(256) metric_stage2_kernel(const double* __restrict__ part, int nb, double* __restrict__ out) {
+  __shared__ double sh[256];
+  const double* __restrict__ p = part + (size_t)blockIdx.x * kMetricMaxBlocks;
+  double s = 0.;
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) s += p[i];
+  sh[threadIdx.x] = s;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) { if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o]; __syncthreads(); }
+  if (threadIdx.x == 0) out[blockIdx.x] = sh[0];
+}
+
 // ---- the leaf loop on the device: the state SerialTreeLearner::Train keeps on the host (leaf ranges and sums, best split per leaf,
 // the growing tree; serial_tree_learner.cpp:159-209, tree.h:533-575) lives in HBM, one thread advances it between the data-parallel
 // kernels, and the host enqueues the kernels of the splits without reading anything back per split.
@@ -856,6 +918,10 @@ struct gpbdev_tree {
   gpbdev_allreduce_fn allreduce = nullptr;
   void* allreduce_ctx = nullptr;
   int64_t n_global = 0;
+  // validation data (lazy): one tree's nodes (L int4 {feature, threshold bin, left, right}) followed by its L leaf values; the metric
+  // kernel's block partials (kMetricAcc x kMetricMaxBlocks, then kMetricAcc results)
+  int4* vnodes_dev = nullptr;
+  double* metric_part = nullptr;
 };
 
 namespace {
@@ -983,6 +1049,7 @@ int gpbdev_tree_free(gpbdev_tree_t h) {
   cudaFree(h->state_dev); cudaFreeHost(h->state_host); cudaFree(h->work_dev);
   cudaFree(h->flag8); cudaFree(h->seg_left);
   cudaFreeHost(h->scalar_host);
+  cudaFree(h->vnodes_dev); cudaFree(h->metric_part);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return 0;
@@ -1268,6 +1335,57 @@ int gpbdev_vec_copy(gpbdev_tree_t h, double* dst_dev, const double* src_dev, int
   if (!h || !dst_dev || !src_dev) return tfail("gpbdev_vec_copy: null argument");
   TCUDA(cudaSetDevice(h->device));
   TCUDA(cudaMemcpyAsync(dst_dev, src_dev, sizeof(double) * n, cudaMemcpyDeviceToDevice, h->stream));
+  return 0;
+}
+
+int gpbdev_tree_valid_add_score(gpbdev_tree_t h, const uint8_t* bins_dev, int Fpad, int64_t nrow, int num_leaves,
+                                const int32_t* split_feature_inner, const int32_t* threshold_bin, const int32_t* left_child,
+                                const int32_t* right_child, const double* leaf_value, double* score_dev) {
+  if (!h || !leaf_value || !score_dev) return tfail("gpbdev_tree_valid_add_score: null argument");
+  if (nrow <= 0) return 0;
+  TCUDA(cudaSetDevice(h->device));
+  const int grid = (int)std::min<int64_t>((nrow + 255) / 256, (int64_t)h->num_sms * 16);
+  if (num_leaves <= 1) {  // constant tree (Tree::AddPredictionToScore with one leaf: the leaf value on every row)
+    add_const_kernel<<<grid, 256, 0, h->stream>>>(score_dev, leaf_value[0], nrow);
+    TCUDA(cudaGetLastError());
+    h->launches += 1;
+    return 0;
+  }
+  if (!bins_dev || !split_feature_inner || !threshold_bin || !left_child || !right_child) return tfail("gpbdev_tree_valid_add_score: null argument");
+  if (num_leaves > h->L) return tfail("gpbdev_tree_valid_add_score: the tree has more leaves than the learner's num_leaves");
+  if (Fpad < h->F) return tfail("gpbdev_tree_valid_add_score: the bin matrix has fewer features than the learner");
+  if (!h->vnodes_dev) TCUDA(cudaMalloc(&h->vnodes_dev, (size_t)h->L * (sizeof(int4) + sizeof(double))));
+  std::vector<int4> nodes(num_leaves - 1);
+  for (int i = 0; i < num_leaves - 1; ++i) {
+    if (split_feature_inner[i] < 0 || split_feature_inner[i] >= h->F) return tfail("gpbdev_tree_valid_add_score: split feature out of range");
+    for (int c : {left_child[i], right_child[i]})
+      if (c >= 0 ? (c <= i || c >= num_leaves - 1) : (~c >= num_leaves)) return tfail("gpbdev_tree_valid_add_score: child index out of range");
+    nodes[i] = make_int4(split_feature_inner[i], threshold_bin[i], left_child[i], right_child[i]);
+  }
+  double* leaf_dev = reinterpret_cast<double*>(h->vnodes_dev + h->L);
+  TCUDA(cudaMemcpyAsync(h->vnodes_dev, nodes.data(), sizeof(int4) * (num_leaves - 1), cudaMemcpyHostToDevice, h->stream));
+  TCUDA(cudaMemcpyAsync(leaf_dev, leaf_value, sizeof(double) * num_leaves, cudaMemcpyHostToDevice, h->stream));
+  valid_tree_score_kernel<<<grid, 256, 0, h->stream>>>(bins_dev, Fpad, nrow, h->vnodes_dev, leaf_dev, score_dev);
+  TCUDA(cudaGetLastError());
+  h->launches += 1;
+  TCUDA(cudaStreamSynchronize(h->stream));  // `nodes` is a temporary; the next tree reuses the node buffer
+  return 0;
+}
+
+int gpbdev_metric_sums(gpbdev_tree_t h, const double* score_dev, const double* label_dev, int64_t n, const double* gp_mean_dev,
+                       const double* gp_dvar_dev, double sigma2, double shift, double* out4) {
+  if (!h || !score_dev || !label_dev || !out4) return tfail("gpbdev_metric_sums: null argument");
+  if (n <= 0) return tfail("gpbdev_metric_sums: no rows");
+  TCUDA(cudaSetDevice(h->device));
+  if (!h->metric_part) TCUDA(cudaMalloc(&h->metric_part, sizeof(double) * (kMetricAcc * kMetricMaxBlocks + kMetricAcc)));
+  const int nb = (int)std::min<int64_t>(kMetricMaxBlocks, (n + 4095) / 4096);
+  double* res = h->metric_part + kMetricAcc * kMetricMaxBlocks;
+  metric_stage1_kernel<<<nb, 256, 0, h->stream>>>(score_dev, label_dev, n, gp_mean_dev, gp_dvar_dev, sigma2, shift, h->metric_part);
+  metric_stage2_kernel<<<kMetricAcc, 256, 0, h->stream>>>(h->metric_part, nb, res);
+  TCUDA(cudaGetLastError());
+  h->launches += 2;
+  TCUDA(cudaMemcpyAsync(out4, res, sizeof(double) * kMetricAcc, cudaMemcpyDeviceToHost, h->stream));
+  TCUDA(cudaStreamSynchronize(h->stream));
   return 0;
 }
 

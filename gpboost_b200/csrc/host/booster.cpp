@@ -1,6 +1,7 @@
 #include "booster.h"
 
 #include <algorithm>
+#include <cctype>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -13,7 +14,49 @@
 namespace gpb200 {
 
 namespace {
+constexpr double kLog2Pi = 1.8378770664093454835606594728112;  // LOG_2PI_ of the reference's metrics
 [[noreturn]] void Fatal(const std::string& m) { throw std::runtime_error(m); }
+// ParseMetricAlias (include/LightGBM/config.h:1262-1271) for the regression metrics; other names pass through unchanged
+std::string MetricAlias(const std::string& t) {
+  if (t == "regression" || t == "regression_l2" || t == "l2" || t == "mean_squared_error" || t == "mse") return "l2";
+  if (t == "l2_root" || t == "root_mean_squared_error" || t == "rmse") return "rmse";
+  if (t == "regression_l1" || t == "l1" || t == "mean_absolute_error" || t == "mae") return "l1";
+  if (t == "none" || t == "null" || t == "custom" || t == "na") return "custom";
+  return t;
+}
+// Config::GetMetricType + ParseMetrics (config.cpp:68-79, :90-109): comma-separated, lower case, aliases resolved, duplicates dropped;
+// "custom" (none / null / na) creates no metric (Metric::CreateMetric). Without a metric: test_neg_log_likelihood with a GP model, else
+// the objective's metric when an objective is given
+std::vector<std::string> ParseMetricList(const Params& p, bool has_gp_model) {
+  auto it = p.kv.find("metric");
+  std::string value = it == p.kv.end() ? std::string() : it->second;
+  for (auto& c : value) c = (char)std::tolower((unsigned char)c);
+  std::vector<std::string> out;
+  auto parse = [&](const std::string& v) {
+    std::string tok;
+    std::istringstream is(v);
+    while (std::getline(is, tok, ',')) {
+      const std::string t = MetricAlias(tok);
+      if (std::find(out.begin(), out.end(), t) == out.end()) out.push_back(t);
+    }
+  };
+  parse(value);
+  if (out.empty() && value.empty()) {
+    if (has_gp_model) {
+      parse("test_neg_log_likelihood");
+    } else {
+      auto ob = p.kv.find("objective");
+      if (ob != p.kv.end()) {
+        std::string o = ob->second;
+        for (auto& c : o) c = (char)std::tolower((unsigned char)c);
+        parse(o);
+      }
+    }
+  }
+  out.erase(std::remove(out.begin(), out.end(), std::string("custom")), out.end());
+  return out;
+}
+bool MetricSupported(const std::string& m) { return m == "l2" || m == "rmse" || m == "l1" || m == "test_neg_log_likelihood"; }
 void TreeCheck(int rc) {
   if (rc != 0) Fatal(std::string(gpbdev_tree_last_error()));
 }
@@ -74,6 +117,12 @@ Booster::Booster(const Dataset* train, const char* parameters, REModel* re_model
   boost_from_average_ = params_.GetBool("boost_from_average", true);
   train_gp_model_cov_pars_ = params_.GetBool("train_gp_model_cov_pars", true);
   params_.RejectUnsupported("Booster");
+  metrics_ = ParseMetricList(params_, re_model_ != nullptr);
+  use_gp_model_for_validation_ = params_.GetBool("use_gp_model_for_validation", true);
+  // read by the Python package's early stopping (callback.early_stopping); parsed here so that a malformed value fails at creation
+  (void)params_.GetInt("early_stopping_round", 0, {"early_stopping_rounds", "early_stopping", "n_iter_no_change"});
+  (void)params_.GetBool("first_metric_only", false);
+  (void)params_.GetInt("metric_freq", 1, {"output_freq"});
   leaves_newton_update_ = params_.GetBool("leaves_newton_update", false);
   if (leaves_newton_update_ && re_model_ == nullptr)
     Fatal("leaves_newton_update can only be 'true' if Gaussian process boosting is done ");  // c_api.cpp:226-228
@@ -215,6 +264,10 @@ Booster::~Booster() {
     gpbdev_vec_free(learner_, grad_dev_);
     if (new_score_dev_) gpbdev_vec_free(learner_, new_score_dev_);
     if (new_score_aux_dev_) gpbdev_vec_free(learner_, new_score_aux_dev_);
+    for (auto& v : valid_) {
+      gpbdev_vec_free(learner_, v.score_dev);
+      gpbdev_vec_free(learner_, v.label_dev);
+    }
     gpbdev_tree_free(learner_);
   }
 }
@@ -247,8 +300,12 @@ bool Booster::TrainOneIter() {
     double suml = 0.;
     for (int64_t i = 0; i < n_; ++i) suml += train_->label()[i];
     init_score = suml / (double)n_;
-    if (std::fabs(init_score) > (double)1e-15f) TreeCheck(gpbdev_vec_add_const(learner_, score_dev_, init_score, n_));
-    else init_score = 0.;
+    if (std::fabs(init_score) > (double)1e-15f) {
+      TreeCheck(gpbdev_vec_add_const(learner_, score_dev_, init_score, n_));
+      for (auto& v : valid_) TreeCheck(gpbdev_vec_add_const(learner_, v.score_dev, init_score, v.n));  // gbdt.cpp:390-395
+    } else {
+      init_score = 0.;
+    }
   }
   if (re_model_ == nullptr || iter_ == 0 || !gradients_ready_) Boosting();  // gbdt.cpp:428-436
   auto tree = std::make_unique<Tree>();
@@ -306,6 +363,7 @@ bool Booster::TrainOneIter() {
   tree->shrinkage = step * learning_rate_;
   TreeCheck(gpbdev_tree_add_score(learner_, tree->leaf_value.data(), nl, score_dev_ + row_begin_, nullptr));  // UpdateScore
   if (sharded_) TreeCheck(gpbdev_vec_allgather_rows(learner_, score_dev_, n_, row_begin_, row_end_));  // scores stay replicated
+  for (auto& v : valid_) AddTreeToValid(*tree, v);  // GBDT::UpdateScore (gbdt.cpp:606-627): the shrunk tree, before AddBias
   if (std::fabs(init_score) > (double)1e-15f) {  // Tree::AddBias (tree.h): stored model only
     for (int i = 0; i < nl; ++i) tree->leaf_value[i] += init_score;
     tree->shrinkage = 1.;
@@ -315,6 +373,125 @@ bool Booster::TrainOneIter() {
   models_.push_back(std::move(tree));
   ++iter_;
   return false;
+}
+
+// ---- validation data ------------------------------------------------------------------------------------------------------
+void Booster::AddTreeToValid(const Tree& t, const ValidSet& v) {
+  TreeCheck(gpbdev_tree_valid_add_score(learner_, v.data->bins_device(), v.data->bins_row_stride(), v.n, t.num_leaves,
+                                        t.split_feature_inner.data(), t.threshold_bin.data(), t.left_child.data(), t.right_child.data(),
+                                        t.leaf_value.data(), v.score_dev));
+}
+
+void Booster::CheckMetricsSupported() const {
+  for (const auto& m : metrics_)
+    if (!MetricSupported(m))
+      Fatal("Metric '" + m + "' is not supported by the CUDA booster (supported: l2, rmse, l1, test_neg_log_likelihood)");
+  if (re_model_ != nullptr && use_gp_model_for_validation_ && !metrics_.empty()) {
+    const std::string why = re_model_->ValidationPredictionUnsupportedReason();
+    if (!why.empty()) Fatal("use_gp_model_for_validation = true: " + why);
+  }
+}
+
+// Booster::AddValidData (c_api.cpp:427-440) -> GBDT::AddValidDataset (gbdt.cpp:159-192): scores of the trees trained so far (the first
+// tree carries the initial score), kept up to date by every later iteration
+void Booster::AddValidData(const Dataset* valid) {
+  if (learner_ == nullptr) Fatal("This Booster was loaded from a model string / file and has no training data (prediction only)");
+  if (valid == nullptr) Fatal("Validation data is null");
+  if (sharded_) Fatal("Validation data is not supported for a row-sharded (data-parallel) booster yet");
+  if (!valid->has_label()) Fatal("The validation Dataset has no label (LGBM_DatasetSetField \"label\")");
+  if (!train_->CheckAlign(*valid)) Fatal("Cannot add validation data, since it has different bin mappers with training data");
+  if (valid->bins_device_id() != train_->bins_device_id()) Fatal("The validation Dataset was binned on another device than the training data");
+  CheckMetricsSupported();
+  ValidSet v;
+  v.data = valid;
+  v.n = valid->num_data();
+  (void)valid->bins_device();  // throws when the Dataset holds no device bins
+  TreeCheck(gpbdev_vec_alloc(learner_, &v.score_dev, v.n));
+  if (gpbdev_vec_alloc(learner_, &v.label_dev, v.n) != 0) {
+    gpbdev_vec_free(learner_, v.score_dev);
+    Fatal(gpbdev_tree_last_error());
+  }
+  std::vector<double> lab(v.n);
+  for (int64_t i = 0; i < v.n; ++i) lab[i] = (double)valid->label()[i];
+  try {
+    TreeCheck(gpbdev_vec_upload(learner_, v.label_dev, lab.data(), v.n));
+    for (const auto& t : models_) AddTreeToValid(*t, v);
+  } catch (...) {
+    gpbdev_vec_free(learner_, v.score_dev);
+    gpbdev_vec_free(learner_, v.label_dev);
+    throw;
+  }
+  valid_.push_back(v);
+}
+
+void Booster::MetricSums(const double* score_dev, const double* label_dev, int64_t n, const double* gp_mean, const double* gp_dvar,
+                         double sigma2, double shift, double* out4) const {
+  TreeCheck(gpbdev_metric_sums(learner_, score_dev, label_dev, n, gp_mean, gp_dvar, sigma2, shift, out4));
+}
+
+// GBDT::GetEvalAt (gbdt.cpp:691-712) with RegressionMetric::Eval (l2, rmse, l1: regression_metric.hpp:28-190) and
+// TestNegLogLikelihood::Eval (:401-479), no weights
+std::vector<double> Booster::GetEval(int data_idx) {
+  if (learner_ == nullptr) Fatal("This Booster was loaded from a model string / file and has no training data (prediction only)");
+  if (data_idx < 0 || data_idx > (int)valid_.size()) Fatal("Check failed: data_idx >= 0 && data_idx <= valid_score_updater_.size()");
+  std::vector<double> ret;
+  if (metrics_.empty()) return ret;
+  for (const auto& m : metrics_)
+    if (!MetricSupported(m)) Fatal("Metric '" + m + "' is not supported by the CUDA booster (supported: l2, rmse, l1, test_neg_log_likelihood)");
+  const bool with_gp = re_model_ != nullptr && use_gp_model_for_validation_;
+  if (data_idx == 0) {
+    for (const auto& m : metrics_) {
+      if (m == "test_neg_log_likelihood") Fatal("Cannot use the metric 'test_neg_log_likelihood' on the training data ");
+      if (with_gp)
+        Fatal("Cannot use the option 'use_gp_model_for_validation = true' for calculating this validation metric on the training data. "
+              "If you want a metric on the training data, either (i) set 'use_gp_model_for_validation = false' or (ii) choose the metric "
+              "'neg_log_likelihood' and use only the training data as validation data.");
+    }
+  }
+  const double* score = data_idx == 0 ? score_dev_ : valid_[data_idx - 1].score_dev;
+  const double* label = data_idx == 0 ? label_dev_ : valid_[data_idx - 1].label_dev;
+  const int64_t n = data_idx == 0 ? n_ : valid_[data_idx - 1].n;
+  const double* gp_mean = nullptr;
+  const double* gp_dvar = nullptr;
+  double sigma2 = 1.;
+  if (with_gp) {
+    CheckMetricsSupported();
+    // the GP predicts from the response F - y that every boosting iteration leaves in the engine (gbdt.cpp:543-550)
+    if (models_.empty()) Fatal("use_gp_model_for_validation = true: the GP model predicts from F - y, which exists after the first boosting iteration");
+    TreeCheck(gpbdev_tree_sync(learner_));
+    re_model_->PredictSavedDevice(n, &gp_mean, &gp_dvar, &sigma2);
+  }
+  double sums[4];
+  MetricSums(score, label, n, gp_mean, gp_dvar, sigma2, 0., sums);
+  double residual_variance = 0.;
+  if (!with_gp && std::find(metrics_.begin(), metrics_.end(), "test_neg_log_likelihood") != metrics_.end()) {
+    // residual variance of the training data (gbdt.cpp:525-542): mean of label - score, then the centred sum of squares
+    double tr[4];
+    MetricSums(score_dev_, label_dev_, n_, nullptr, nullptr, 1., 0., tr);
+    const double residual_mean = -tr[2] / (double)n_;  // sum (label - score) = -sum (score - label)
+    MetricSums(score_dev_, label_dev_, n_, nullptr, nullptr, 1., residual_mean, tr);  // sum (score - label + mean)^2
+    residual_variance = tr[0] / (double)(n_ - 1);
+  }
+  const double dn = (double)n;
+  for (const auto& m : metrics_) {
+    if (m == "l2") ret.push_back(sums[0] / dn);
+    else if (m == "rmse") ret.push_back(std::sqrt(sums[0] / dn));
+    else if (m == "l1") ret.push_back(sums[1] / dn);
+    else if (with_gp) ret.push_back(0.5 * (sums[3] + dn * kLog2Pi) / dn);
+    else ret.push_back(0.5 * (sums[0] / residual_variance + dn * std::log(residual_variance) + dn * kLog2Pi) / dn);
+  }
+  return ret;
+}
+
+int64_t Booster::NumPredict(int data_idx) const {
+  if (data_idx < 0 || data_idx > (int)valid_.size()) Fatal("Check failed: data_idx >= 0 && data_idx <= valid_score_updater_.size()");
+  return data_idx == 0 ? n_ : valid_[data_idx - 1].n;
+}
+
+void Booster::GetPredict(int data_idx, double* out) {  // GBDT::GetPredictAt (gbdt.cpp:745-780): raw scores (L2: ConvertOutput is identity)
+  if (data_idx == 0) { GetTrainingScore(out); return; }
+  const int64_t n = NumPredict(data_idx);
+  TreeCheck(gpbdev_vec_download(learner_, out, valid_[data_idx - 1].score_dev, n));
 }
 
 void Booster::TimeRootHistogram(int reps, float* mean_ms, int* row_bytes, int64_t* rows) const {

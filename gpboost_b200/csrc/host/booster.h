@@ -57,11 +57,32 @@ class Booster {
   std::vector<double> FeatureImportance(int num_iteration, int importance_type) const;
   double LeafValue(int tree_idx, int leaf_idx) const;
   gpbdev_tree_t learner() const { return learner_; }
+  // ---- validation data and metrics (Booster::AddValidData, c_api.cpp:427-440; GBDT::AddValidDataset / GetEvalAt / GetPredictAt,
+  // gbdt.cpp:159-192, :691-712, :745-780). Data index 0 is the training data, k >= 1 the k-th validation set.
+  void AddValidData(const Dataset* valid);
+  const std::vector<std::string>& metric_names() const { return metrics_; }
+  std::vector<double> GetEval(int data_idx);
+  int64_t NumPredict(int data_idx) const;
+  void GetPredict(int data_idx, double* out);
   // bench hook: mean device time of the root-pass histogram kernel on this rank's rows with the current gradient (bench.py roofline)
   void TimeRootHistogram(int reps, float* mean_ms, int* row_bytes, int64_t* rows) const;
 
  private:
   void Boosting();  // gradients for the next tree (+ covariance-parameter fit when a GP model is attached)
+  struct ValidSet {
+    const Dataset* data = nullptr;
+    int64_t n = 0;
+    double* score_dev = nullptr;  // raw scores of the ensemble so far (ScoreUpdater)
+    double* label_dev = nullptr;
+  };
+  void AddTreeToValid(const Tree& tree, const ValidSet& v);
+  void CheckMetricsSupported() const;
+  // metric sums of (score, label) over n rows (gpbdev_metric_sums), optionally with the GP's prediction
+  void MetricSums(const double* score_dev, const double* label_dev, int64_t n, const double* gp_mean, const double* gp_dvar, double sigma2,
+                  double shift, double* out4) const;
+  std::vector<ValidSet> valid_;
+  std::vector<std::string> metrics_;        // canonical names (Config::GetMetricType, config.cpp:90-109)
+  bool use_gp_model_for_validation_ = true;  // config.h:187
   const Dataset* train_ = nullptr;
  public:
   const Dataset* train_data() const { return train_; }

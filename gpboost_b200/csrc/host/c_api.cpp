@@ -235,8 +235,11 @@ int GPB_CanCalculateStandardErrorsCovPars(REModelHandle handle, int* out) {
 int LGBM_DatasetCreateFromMat(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, const char* parameters,
                               const DatasetHandle reference, DatasetHandle* out) {
   API_BEGIN();
-  if (reference != nullptr) throw std::runtime_error("LGBM_DatasetCreateFromMat: 'reference' datasets are not supported by this build yet");
-  *out = new gpb200::Dataset(data, data_type, nrow, ncol, is_row_major, gpb200::Params::Parse(parameters));
+  if (reference != nullptr)  // validation data: the reference's bin mappers (c_api.cpp:1134-1160)
+    *out = new gpb200::Dataset(data, data_type, nrow, ncol, is_row_major, gpb200::Params::Parse(parameters),
+                               *reinterpret_cast<const gpb200::Dataset*>(reference));
+  else
+    *out = new gpb200::Dataset(data, data_type, nrow, ncol, is_row_major, gpb200::Params::Parse(parameters));
   API_END();
 }
 
@@ -313,18 +316,38 @@ int LGBM_BoosterNumberOfTotalModel(BoosterHandle handle, int* out_models) {
   API_END();
 }
 
+// data_idx 0: training data, k >= 1: the k-th validation set (GBDT::GetPredictAt, gbdt.cpp:745-780): raw scores
 int LGBM_BoosterGetNumPredict(BoosterHandle handle, int data_idx, int64_t* out_len) {
   API_BEGIN();
-  if (data_idx != 0) throw std::runtime_error("Only the training data (data_idx = 0) is available in this build");
-  *out_len = B(handle)->num_data();
+  *out_len = B(handle)->NumPredict(data_idx);
   API_END();
 }
 
 int LGBM_BoosterGetPredict(BoosterHandle handle, int data_idx, int64_t* out_len, double* out_result) {
   API_BEGIN();
-  if (data_idx != 0) throw std::runtime_error("Only the training data (data_idx = 0) is available in this build");
-  B(handle)->GetTrainingScore(out_result);
-  *out_len = B(handle)->num_data();
+  B(handle)->GetPredict(data_idx, out_result);
+  *out_len = B(handle)->NumPredict(data_idx);
+  API_END();
+}
+
+int LGBM_BoosterAddValidData(BoosterHandle handle, const DatasetHandle valid_data) {
+  API_BEGIN();
+  B(handle)->AddValidData(reinterpret_cast<const gpb200::Dataset*>(valid_data));
+  API_END();
+}
+
+// one value per configured metric, in the order of LGBM_BoosterGetEvalNames (GBDT::GetEvalAt, gbdt.cpp:691-712)
+int LGBM_BoosterGetEval(BoosterHandle handle, int data_idx, int* out_len, double* out_results) {
+  API_BEGIN();
+  const std::vector<double> r = B(handle)->GetEval(data_idx);
+  for (size_t i = 0; i < r.size(); ++i) out_results[i] = r[i];
+  *out_len = (int)r.size();
+  API_END();
+}
+
+int LGBM_BoosterGetEvalCounts(BoosterHandle handle, int* out_len) {
+  API_BEGIN();
+  *out_len = (int)B(handle)->metric_names().size();
   API_END();
 }
 
@@ -462,10 +485,10 @@ int LGBM_BoosterCalcNumPredict(BoosterHandle handle, int num_row, int predict_ty
   API_END();
 }
 
-int LGBM_BoosterGetEvalNames(BoosterHandle handle, const int /*len*/, int* out_len, const size_t /*buffer_len*/, size_t* out_buffer_len, char** /*out_strs*/) {
+// the configured metrics (Booster::GetEvalNames, c_api.cpp:893-908)
+int LGBM_BoosterGetEvalNames(BoosterHandle handle, const int len, int* out_len, const size_t buffer_len, size_t* out_buffer_len, char** out_strs) {
   API_BEGIN();
-  B(handle);
-  *out_len = 0; *out_buffer_len = 0;  // no metric is evaluated by the CUDA booster
+  CopyNames(B(handle)->metric_names(), len, out_len, buffer_len, out_buffer_len, out_strs);
   API_END();
 }
 

@@ -110,13 +110,6 @@ int GPB_SetOffsetData(REModelHandle handle, const double* fixed_effects) {
   API_END();
 }
 
-int LGBM_BoosterAddValidData(BoosterHandle handle, const DatasetHandle valid_data) {
-  API_BEGIN();
-  (void)handle; (void)valid_data;
-  Unsupported("LGBM_BoosterAddValidData");
-  API_END();
-}
-
 int LGBM_BoosterDumpModel(BoosterHandle handle, int start_iteration, int num_iteration, int feature_importance_type, int64_t buffer_len, int64_t* out_len, char* out_str) {
   API_BEGIN();
   (void)handle; (void)start_iteration; (void)num_iteration; (void)feature_importance_type; (void)buffer_len; (void)out_len; (void)out_str;
@@ -128,19 +121,6 @@ int LGBM_BoosterFreePredictSparse(void* indptr, int32_t* indices, void* data, in
   API_BEGIN();
   (void)indptr; (void)indices; (void)data; (void)indptr_type; (void)data_type;
   Unsupported("LGBM_BoosterFreePredictSparse");
-  API_END();
-}
-
-int LGBM_BoosterGetEval(BoosterHandle handle, int data_idx, int* out_len, double* out_results) {
-  API_BEGIN();
-  (void)handle; (void)data_idx; (void)out_len; (void)out_results;
-  Unsupported("LGBM_BoosterGetEval");
-  API_END();
-}
-
-int LGBM_BoosterGetEvalCounts(BoosterHandle handle, int* out_len) {
-  API_BEGIN();
-  (void)handle; *out_len = 0;  // no metric is evaluated by the CUDA booster
   API_END();
 }
 

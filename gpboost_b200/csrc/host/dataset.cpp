@@ -232,6 +232,7 @@ static const std::map<std::string, std::string>& AliasTable() {
       {"subsample_for_bin", "bin_construct_sample_cnt"}, {"data_seed", "data_random_seed"},
       {"cat_feature", "categorical_feature"}, {"categorical_column", "categorical_feature"}, {"cat_column", "categorical_feature"},
       {"num_classes", "num_class"}, {"unbalance", "is_unbalance"}, {"unbalanced_sets", "is_unbalance"},
+      {"metrics", "metric"}, {"metric_types", "metric"},
   };
   return t;
 }
@@ -344,6 +345,40 @@ Dataset::Dataset(const void* data, int data_type, int32_t nrow, int32_t ncol, in
     if (bins_[j].num_bin < 0) Fatal("Missing values (NaN) in the feature matrix are not supported by the CUDA tree learner yet");
   for (int j = 0; j < ncol; ++j)
     if (!bins_[j].trivial) used_features_.push_back(j);
+  BinOnDevice(data, data_type, nrow, ncol, is_row_major);
+}
+
+// Validation data (LGBM_DatasetCreateFromMat with a reference, c_api.cpp:1134-1160 -> DatasetLoader::ConstructFromSampleData with the
+// reference's bin mappers): the training data's boundaries and feature set, so that the trees' bin thresholds apply to these rows
+// (Dataset::CheckAlign, dataset.h). The values are binned on the device like the training data's.
+Dataset::Dataset(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, const Params& params, const Dataset& reference)
+    : num_data_(nrow), num_total_features_(ncol), params_(params) {
+  if (data == nullptr || nrow <= 0 || ncol <= 0) Fatal("LGBM_DatasetCreateFromMat: empty data");
+  if (data_type != 0 && data_type != 1) Fatal("Unknown data type in LGBM_DatasetCreateFromMat (float32 / float64 supported)");
+  params.RejectUnsupported("Dataset");
+  if (ncol != reference.num_total_features())
+    Fatal("The number of features of the data (" + std::to_string(ncol) + ") differs from the reference Dataset's (" +
+          std::to_string(reference.num_total_features()) + ")");
+  for (int64_t i = 0; i < (int64_t)nrow * ncol; ++i) {
+    const double v = data_type == 0 ? (double)static_cast<const float*>(data)[i] : static_cast<const double*>(data)[i];
+    if (std::isnan(v)) Fatal("Missing values (NaN) in the feature matrix are not supported by the CUDA tree learner yet");
+  }
+  bins_ = reference.bins_;
+  used_features_ = reference.used_features_;
+  feature_names_ = reference.feature_names_;
+  BinOnDevice(data, data_type, nrow, ncol, is_row_major);
+}
+
+bool Dataset::CheckAlign(const Dataset& other) const {  // Dataset::CheckAlign (include/LightGBM/dataset.h): same features, same bins
+  if (num_total_features_ != other.num_total_features_ || used_features_ != other.used_features_) return false;
+  for (int real : used_features_) {
+    const FeatureBins &a = bins_[real], &b = other.bins_[real];
+    if (a.num_bin != b.num_bin || a.upper_bounds != b.upper_bounds) return false;
+  }
+  return true;
+}
+
+void Dataset::BinOnDevice(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major) {
   // ---- value -> bin for every row: on the device, straight into the learner's row-major layout (csrc/dev/binning.cu)
   const int F = (int)used_features_.size();
   if (F == 0) return;

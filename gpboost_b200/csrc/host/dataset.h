@@ -43,7 +43,11 @@ class Dataset {
  public:
   // data: nrow x ncol, float32 or float64 (C_API_DTYPE_*), row- or column-major
   Dataset(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, const Params& params);
+  // binned with the bin mappers (feature set, upper bounds) of `reference` (validation data: LGBM_DatasetCreateFromMat with a reference)
+  Dataset(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, const Params& params, const Dataset& reference);
   ~Dataset();
+  // same feature set and bin boundaries (Dataset::CheckAlign): the trees of one can be walked on the bins of the other
+  bool CheckAlign(const Dataset& other) const;
   Dataset(const Dataset&) = delete;
   Dataset& operator=(const Dataset&) = delete;
   int32_t num_data() const { return num_data_; }
@@ -68,6 +72,7 @@ class Dataset {
   std::vector<std::string> feature_infos() const;
 
  private:
+  void BinOnDevice(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major);
   int32_t num_data_ = 0;
   int num_total_features_ = 0;
   Params params_;

@@ -167,6 +167,7 @@ REModel::REModel(int32_t num_data, const int32_t* cluster_ids_data, const char* 
 }
 
 REModel::~REModel() {
+  if (predset_) gpbdev_vecchia_predset_free(predset_);
   if (engine_) gpbdev_vecchia_free(engine_);
   if (grouped_) gpbdev_grouped_free(grouped_);
   if (dense_) gpbdev_dense_free(dense_);
@@ -571,6 +572,10 @@ void REModel::EvalNegLogLikelihood(const double* y_data, const double* cov_pars,
 void REModel::SetPredictionData(int32_t num_data_pred, const double* gp_coords_data_pred, const double* covariate_data_pred,
                                 const char* vecchia_pred_type, int num_neighbors_pred) {
   if (engine_ == nullptr) Fatal("Prediction data can only be set for a Vecchia GP model in this build");
+  if (predset_) {  // the validation prediction set belongs to the previous locations / neighbour count
+    gpbdev_vecchia_predset_free(predset_);
+    predset_ = nullptr;
+  }
   if (covariate_data_pred != nullptr) {
     if (num_covariates_ == 0) Fatal("Covariate data provided for prediction but the model has no linear regression covariates");
     if (!(num_data_pred > 0)) Fatal("Check failed: num_data_pred > 0");
@@ -659,6 +664,30 @@ void REModel::Predict(const double* y_obs, int32_t num_data_pred, double* out_pr
     const double add = predict_response ? 1. : 0.;
     for (int32_t i = 0; i < num_data_pred; ++i) out_predict[(size_t)num_data_pred + i] = trans[0] * (dvar[(size_t)i] + add);
   }
+}
+
+std::string REModel::ValidationPredictionUnsupportedReason() const {
+  if (engine_ == nullptr)
+    return "the grouped and exact GP models cannot predict in this build yet: set use_gp_model_for_validation=False to validate on the "
+           "tree ensemble's scores";
+  if (!gauss_) return "prediction is not supported for likelihood '" + likelihood_ + "' by the CUDA engine yet";
+  if (num_covariates_ > 0) return "a GP model with linear regression covariates cannot be used for validation in the GPBoost algorithm";
+  return "";
+}
+
+void REModel::PredictSavedDevice(int64_t num_rows, const double** mean_dev, const double** dvar_dev, double* sigma2) {
+  const std::string why = ValidationPredictionUnsupportedReason();
+  if (!why.empty()) Fatal("use_gp_model_for_validation: " + why);
+  if (num_data_pred_saved_ <= 0)
+    Fatal("Prediction data of the GP model is needed for 'use_gp_model_for_validation = true': call set_prediction_data "
+          "(GPModel.set_prediction_data(gp_coords_pred=...)) with the coordinates of the validation data");
+  if (num_rows != num_data_pred_saved_)
+    Fatal("The number of rows of the validation data (" + std::to_string(num_rows) + ") differs from the number of points of the GP's "
+          "prediction data (" + std::to_string(num_data_pred_saved_) + ") set with set_prediction_data");
+  if (!cov_pars_initialized_) Fatal("Covariance parameters have not been estimated or are not given.");
+  if (predset_ == nullptr) DevCheck(gpbdev_vecchia_predset_create(engine_, coords_pred_saved_.data(), num_data_pred_saved_, num_neighbors_pred_, &predset_));
+  DevCheck(gpbdev_vecchia_predset_eval(predset_, cov_id_, cov_pars_[1], cov_pars_[2], mean_dev, dvar_dev));
+  *sigma2 = cov_pars_[0];
 }
 
 void REModel::OptimCovPar(const double* y_data, const double* fixed_effects, bool called_in_GPBoost_algorithm,

@@ -80,6 +80,14 @@ class REModel {
   void Predict(const double* y_obs, int32_t num_data_pred, double* out_predict, bool predict_cov_mat, bool predict_var,
                bool predict_response, const double* gp_coords_data_pred, const double* cov_pars_pred, bool use_saved_data,
                const double* fixed_effects, const double* covariate_data_pred = nullptr);
+  // Validation data of the boosting loop (RegressionMetric::Eval -> REModel::Predict(use_saved_data, suppress_calc_cov_factor),
+  // regression_metric.hpp:92-104, :427-440): the GP's prediction at the locations of GPB_SetPredictionData from the engine's current
+  // response (F - y after every boosting iteration: the caller has run one) at the current covariance parameters. The prediction set (locations and neighbour
+  // sets in HBM) is built on the first call after GPB_SetPredictionData. Device pointers to num_rows means and D_p values (transformed
+  // scale, valid until the next call); *sigma2 = the error variance that scales D_p. Returns once the results are complete.
+  void PredictSavedDevice(int64_t num_rows, const double** mean_dev, const double** dvar_dev, double* sigma2);
+  // why this model cannot predict validation data with the GP, or "" when PredictSavedDevice works
+  std::string ValidationPredictionUnsupportedReason() const;
   // GPB_GetCovPar / GPB_GetInitCovPar (original scale). With calc_std_dev the standard errors follow in out[num_cov_pars ..
   // 2 num_cov_pars) (REModel::GetCovPar, re_model.cpp:921-965): computed once per fit and cached.
   void GetCovPar(double* out, bool calc_std_dev);
@@ -119,6 +127,7 @@ class REModel {
   int num_neighbors_ = 20;
   int num_neighbors_pred_ = 40;          // 2 x num_neighbors (re_model_template.h:299)
   std::vector<double> coords_pred_saved_;  // np x d row-major (GPB_SetPredictionData)
+  gpbdev_vecchia_predset_t predset_ = nullptr;  // prediction set of coords_pred_saved_ (PredictSavedDevice), freed by GPB_SetPredictionData
   std::vector<double> covariates_pred_saved_;  // np x num_covariates column-major (GPB_SetPredictionData)
   int32_t num_data_pred_saved_ = 0;
   bool y_has_been_set_ = false;

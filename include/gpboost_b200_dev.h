@@ -95,6 +95,21 @@ GPBDEV_EXPORT int gpbdev_vecchia_laplace_time_ops(gpbdev_vecchia_t h, int t, int
  * mean_out_host[p] = A_p y_N(p); var_out_host[p] = D_p on the transformed scale (times sigma^2 = latent predictive variance). */
 GPBDEV_EXPORT int gpbdev_vecchia_predict(gpbdev_vecchia_t h, int cov_type, double var, double range, const double* coords_pred_host,
                                          int64_t np, int num_neighbors_pred, double* mean_out_host, double* var_out_host);
+/* The same prediction split in two, for locations that are predicted at many parameter values or responses (validation data of the
+ * boosting loop, GBDT::OutputMetric -> RegressionMetric::Eval -> REModel::Predict with the saved prediction data,
+ * src/LightGBM/metric/regression_metric.hpp:92-104, :427-440). gpbdev_vecchia_predset_create copies the locations once and runs the
+ * neighbour search once (the part of CalcPredVecchiaObservedFirstOrder that does not depend on the parameters,
+ * Vecchia_utils.cpp:1701-1760); coordinates and neighbour sets stay in HBM. gpbdev_vecchia_predset_eval runs the prediction kernel at
+ * transformed (var, range) on the engine's current response and returns device pointers (np doubles each, valid until the next eval or
+ * free) to mean = A_p y_N(p) and D_p (transformed scale). It returns after the engine's stream has completed, so any stream may read the
+ * results; it does not touch the stored factor, the response or the STORE shortcut. gpbdev_vecchia_predict is create + eval + free.
+ * A prediction set must be freed before its engine. */
+typedef struct gpbdev_vecchia_predset* gpbdev_vecchia_predset_t;
+GPBDEV_EXPORT int gpbdev_vecchia_predset_create(gpbdev_vecchia_t h, const double* coords_pred_host, int64_t np, int num_neighbors_pred,
+                                                gpbdev_vecchia_predset_t* out);
+GPBDEV_EXPORT int gpbdev_vecchia_predset_eval(gpbdev_vecchia_predset_t ps, int cov_type, double var, double range, const double** mean_dev,
+                                              const double** var_dev);
+GPBDEV_EXPORT int gpbdev_vecchia_predset_free(gpbdev_vecchia_predset_t ps);
 /* Newton update of the leaf values in GPBoost (SURVEY §8 f2; REModelTemplate::NewtonUpdateLeafValues, Vecchia branch,
  * include/GPBoost/re_model_template.h:4982-5063). After a STORE pass at the current parameters: M_host (L x L row-major) =
  * H^T B^T D^-1 B H and rhs_host (L) = H^T g for the leaf incidence H given by leaf_of_row_dev (n int32, original row order, device)
@@ -330,6 +345,20 @@ GPBDEV_EXPORT int gpbdev_vec_copy(gpbdev_tree_t h, double* dst_dev, const double
 GPBDEV_EXPORT int gpbdev_tree_set_allreduce(gpbdev_tree_t h, gpbdev_allreduce_fn fn, void* ctx, int64_t n_global);
 /* replicated n-vector of which this rank keeps rows [b, e) current: bring the whole vector up to date on every rank */
 GPBDEV_EXPORT int gpbdev_vec_allgather_rows(gpbdev_tree_t h, double* vec_dev, int64_t n, int64_t b, int64_t e);
+/* Validation data (ScoreUpdater::AddScore(tree), score_updater.hpp:93 -> Tree::AddPredictionToScore, tree.h:104-120):
+ * score_dev[i] += leaf_value[leaf(i)] for every row i of a bin matrix (bins_dev: row-major nrow x Fpad uint8 of a Dataset binned with
+ * the training data's bin mappers), walking the tree with bin <= threshold_bin -> left. Per internal node (num_leaves - 1 entries):
+ * split_feature_inner, threshold_bin, left_child, right_child (~leaf for leaves); leaf_value: num_leaves. num_leaves = 1 adds
+ * leaf_value[0] to every row. num_leaves <= the learner's num_leaves. Enqueued on the learner's stream. */
+GPBDEV_EXPORT int gpbdev_tree_valid_add_score(gpbdev_tree_t h, const uint8_t* bins_dev, int Fpad, int64_t nrow, int num_leaves,
+                                              const int32_t* split_feature_inner, const int32_t* threshold_bin, const int32_t* left_child,
+                                              const int32_t* right_child, const double* leaf_value, double* score_dev);
+/* Fused metric sums over n rows (RegressionMetric::Eval / TestNegLogLikelihood::Eval, regression_metric.hpp:28-190, :401-479), in a
+ * fixed order (repeated calls are bitwise equal). With e_i = (score_i - gp_mean_i) - label_i (gp_mean NULL: e_i = score_i - label_i)
+ * and v_i = sigma2 (gp_dvar_i + 1) (the response variance on the original scale, REModel::Predict): out4 = { sum (e_i + shift)^2,
+ * sum |e_i|, sum e_i, sum e_i^2 / v_i + log v_i (0 without gp_dvar) }. Device inputs; runs on the learner's stream, returns synchronised. */
+GPBDEV_EXPORT int gpbdev_metric_sums(gpbdev_tree_t h, const double* score_dev, const double* label_dev, int64_t n, const double* gp_mean_dev,
+                                     const double* gp_dvar_dev, double sigma2, double shift, double* out4);
 GPBDEV_EXPORT int gpbdev_tree_sync(gpbdev_tree_t h);
 GPBDEV_EXPORT int64_t gpbdev_tree_launch_count(gpbdev_tree_t h);
 GPBDEV_EXPORT void* gpbdev_tree_stream(gpbdev_tree_t h);
