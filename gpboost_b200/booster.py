@@ -9,7 +9,7 @@ from .basic import GPBoostError, c_str, _dptr
 from .libpath import load_lib
 
 C_API_DTYPE_FLOAT32, C_API_DTYPE_FLOAT64 = 0, 1
-C_API_PREDICT_NORMAL, C_API_PREDICT_RAW_SCORE = 0, 1
+C_API_PREDICT_NORMAL, C_API_PREDICT_RAW_SCORE, C_API_PREDICT_LEAF_INDEX, C_API_PREDICT_CONTRIB = 0, 1, 2, 3
 
 
 def _param_value_str(v):
@@ -25,10 +25,14 @@ def param_dict_to_str(params):
 
 
 class Dataset(object):
-    def __init__(self, data, label=None, params=None, reference=None, _lib=None):
-        """`reference`: the training Dataset whose bin mappers bin this one (validation data, Dataset(..., reference=train_set))."""
+    def __init__(self, data, label=None, params=None, reference=None, free_raw_data=True, _lib=None):
+        """`reference`: the training Dataset whose bin mappers bin this one (validation data, Dataset(..., reference=train_set)).
+        `free_raw_data=False` keeps the feature matrix as `self.data` (the library only holds its bins): Booster.predict with a
+        GP model needs it to predict the training data."""
         self._LIB = load_lib() if _lib is None else _lib
         self.reference = reference
+        self.free_raw_data = free_raw_data
+        self.data = None
         data = np.asarray(data)
         # float32 matrices are passed as they are (C_API_DTYPE_FLOAT32), like the reference's package (basic.py: __init_from_np2d)
         dt = np.float32 if data.dtype == np.float32 else np.float64
@@ -41,6 +45,8 @@ class Dataset(object):
             data.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(C_API_DTYPE_FLOAT32 if dt == np.float32 else C_API_DTYPE_FLOAT64), ctypes.c_int32(self.num_data),
             ctypes.c_int32(self.num_feature), ctypes.c_int(1), c_str(param_dict_to_str(params)),
             None if reference is None else reference.handle, ctypes.byref(self.handle)))
+        if not free_raw_data:
+            self.data = data
         if label is not None:
             self.set_label(label)
 
@@ -192,14 +198,77 @@ class Booster(object):
         self._safe_call(self._LIB.LGBM_BoosterGetPredict(self.handle, ctypes.c_int(data_idx), ctypes.byref(n), _dptr(out)))
         return out
 
-    def predict(self, data, raw_score=True, start_iteration=0, num_iteration=-1):
-        data = np.ascontiguousarray(np.asarray(data, dtype=np.float64))
+    def _predict_for_mat(self, data, predict_type, start_iteration, num_iteration):
+        """LGBM_BoosterPredictForMat on a dense matrix (float32 passed as it is, everything else as float64)."""
+        data = np.asarray(data)
+        dt = np.float32 if data.dtype == np.float32 else np.float64
+        data = np.ascontiguousarray(data, dtype=dt)
+        if data.ndim != 2:
+            raise ValueError("'data' needs to be a 2-D array")
         n = ctypes.c_int64(0)
-        out = np.empty(data.shape[0], dtype=np.float64)
+        self._safe_call(self._LIB.LGBM_BoosterCalcNumPredict(self.handle, ctypes.c_int(data.shape[0]), ctypes.c_int(predict_type),
+                                                             ctypes.c_int(start_iteration), ctypes.c_int(num_iteration), ctypes.byref(n)))
+        out = np.empty(n.value, dtype=np.float64)
         self._safe_call(self._LIB.LGBM_BoosterPredictForMat(
-            self.handle, data.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(C_API_DTYPE_FLOAT64), ctypes.c_int32(data.shape[0]),
-            ctypes.c_int32(data.shape[1]), ctypes.c_int(1), ctypes.c_int(C_API_PREDICT_RAW_SCORE if raw_score else C_API_PREDICT_NORMAL),
+            self.handle, data.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(C_API_DTYPE_FLOAT32 if dt == np.float32 else C_API_DTYPE_FLOAT64),
+            ctypes.c_int32(data.shape[0]), ctypes.c_int32(data.shape[1]), ctypes.c_int(1), ctypes.c_int(predict_type),
             ctypes.c_int(start_iteration), ctypes.c_int(num_iteration), c_str(""), ctypes.byref(n), _dptr(out)))
+        if n.value != out.shape[0]:
+            raise ValueError("Wrong length for predict results")
+        if predict_type == C_API_PREDICT_LEAF_INDEX:
+            return out.astype(np.int32).reshape(data.shape[0], out.shape[0] // data.shape[0])
+        return out
+
+    def predict(self, data, start_iteration=0, num_iteration=None, raw_score=None, pred_leaf=False, pred_latent=False, gp_coords_pred=None,
+                predict_var=False, cov_pars=None, ignore_gp_model=False, offset_pred=None, num_neighbors_pred=-1, pred_contrib=False,
+                predict_cov_mat=False, sample_posterior=False):
+        """Prediction at new data (Booster.predict, basic.py:3376-3802). Without a `gp_model` (or with `ignore_gp_model=True`): the
+        tree ensemble's scores, or with `pred_leaf=True` the (nrow, trees) leaf indices. With a Gaussian `gp_model`: the reference's
+        dict — `pred_latent=True`: fixed_effect, random_effect_mean, random_effect_cov (the variances, with `predict_var`);
+        `pred_latent=False`: response_mean, response_var. The GP predicts from the residual label - F(X_train), so the training
+        Dataset must have been built with `free_raw_data=False`. `num_iteration=None` uses `best_iteration`. An explicit `raw_score`
+        (an argument the reference has discontinued) asks for the tree ensemble's scores alone, as it always has here, also with a
+        `gp_model`."""
+        if pred_contrib:
+            raise GPBoostError("Feature contributions (pred_contrib) are not supported by this build")
+        if predict_cov_mat or sample_posterior:
+            raise GPBoostError("Predictive covariance matrices (predict_cov_mat) and posterior samples (sample_posterior) are not supported "
+                               "by this build")
+        if num_iteration is None:  # basic.py:3623-3627
+            num_iteration = self.best_iteration if start_iteration <= 0 else -1
+        if self.gp_model is None or ignore_gp_model or raw_score is not None:
+            ptype = C_API_PREDICT_LEAF_INDEX if pred_leaf else (C_API_PREDICT_NORMAL if raw_score is False else C_API_PREDICT_RAW_SCORE)
+            return self._predict_for_mat(data, ptype, start_iteration, num_iteration)
+        if pred_leaf:
+            raise GPBoostError("pred_leaf with a gp_model is not supported by this build: set ignore_gp_model=True for the leaf indices")
+        if self.train_set is None or getattr(self.train_set, "data", None) is None:
+            raise GPBoostError("Cannot make predictions for Gaussian process. Set free_raw_data = False when you construct the Dataset")
+        if self.gp_model._get_likelihood_name() != "gaussian":
+            raise GPBoostError("Prediction with a gp_model is only supported for the gaussian likelihood by this build (likelihood: %s)"
+                               % self.gp_model._get_likelihood_name())
+        if gp_coords_pred is None:
+            raise GPBoostError("'gp_coords_pred' is needed for the prediction with a gp_model")
+        # basic.py:3646-3700: the GP predicts from the residual of the training data under the same trees
+        fixed_effect_train = self._predict_for_mat(self.train_set.data, C_API_PREDICT_RAW_SCORE, start_iteration, num_iteration)
+        residual = self.train_set.label - fixed_effect_train
+        re_pred = self.gp_model.predict(y=residual, gp_coords_pred=gp_coords_pred, cov_pars=cov_pars, predict_var=predict_var,
+                                        predict_response=not pred_latent, num_neighbors_pred=num_neighbors_pred)
+        fixed_effect = self._predict_for_mat(data, C_API_PREDICT_RAW_SCORE, start_iteration, num_iteration)
+        if len(fixed_effect) != len(re_pred["mu"]):
+            raise GPBoostError("Number of data points in fixed effect (tree ensemble) and random effect are not equal")
+        if offset_pred is not None:
+            offset_pred = np.asarray(offset_pred, dtype=np.float64).reshape(-1)
+            if len(fixed_effect) != len(offset_pred):
+                raise GPBoostError("Number of data points in fixed effect (tree ensemble) and 'offset_pred' are not equal")
+            fixed_effect = fixed_effect + offset_pred
+        out = {"fixed_effect": None, "random_effect_mean": None, "random_effect_cov": None, "response_mean": None, "response_var": None}
+        if pred_latent:
+            out["fixed_effect"] = fixed_effect
+            out["random_effect_mean"] = re_pred["mu"]
+            out["random_effect_cov"] = re_pred["var"] if predict_var else None
+        else:
+            out["response_mean"] = re_pred["mu"] + fixed_effect
+            out["response_var"] = re_pred["var"] if predict_var else None
         return out
 
     def __del__(self):

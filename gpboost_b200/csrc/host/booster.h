@@ -4,6 +4,12 @@
 // the L2 objective with its GP coupling (src/LightGBM/objective/regression_objective.hpp:153-201, :259-290) and Tree's
 // bookkeeping (include/LightGBM/tree.h, src/LightGBM/io/tree.cpp) for: objective=regression, numerical features, no bagging /
 // feature sampling. Trees are grown by the device learner (gpbdev_tree_*); training scores and gradients stay on the device.
+//
+// Prediction on a raw feature matrix (Predict) runs on the device (gpbdev_ensemble_*): the trees are packed lazily, kept in HBM and
+// repacked when a tree was added. Whether a booster predicts on the device is decided once, at construction: a training booster
+// always does (the learner's device); a booster loaded from a model string does when the process sees a CUDA device, and otherwise
+// walks the trees on the host (Tree::PredictLeaf) — the one configuration that works without a device. PredictHost is that walk; besides
+// the device-less model-string booster only the comparison hook GPB200_BoosterPredictForMatHost calls it.
 #ifndef GPB200_BOOSTER_H_
 #define GPB200_BOOSTER_H_
 #include <memory>
@@ -28,7 +34,7 @@ struct Tree {
   std::vector<double> leaf_value;
   std::vector<int> leaf_count;
   double shrinkage = 1.;
-  double Predict(const double* row) const;
+  int PredictLeaf(const double* row) const;  // leaf index of a row of real feature values
   std::string ToString() const;
 };
 
@@ -50,8 +56,16 @@ class Booster {
   // trees [first, first + count) of the ensemble, clamped like GBDT::PredictRaw / SaveModelToString (start_iteration, num_iteration
   // of the C API; num_iteration <= 0: all remaining)
   void IterationRange(int start_iteration, int num_iteration, int* first, int* count) const;
-  void Predict(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, double* out, int start_iteration = 0,
-               int num_iteration = -1) const;
+  // what = 0: out[row] = sum of the leaf values of the trees of the iteration range (raw score); what = 1: out[row * count + k] = leaf
+  // index of the row in the k-th tree of the range (GBDT::PredictLeafIndex)
+  void Predict(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, double* out, int start_iteration,
+               int num_iteration, int what);
+  void PredictHost(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, double* out, int start_iteration,
+                   int num_iteration, int what) const;
+  // test / bench hooks of the device prediction (gpbdev_ensemble_plan, gpbdev_ensemble_time_kernel)
+  void PredictPlan(int data_type, int32_t ncol, int start_iteration, int num_iteration, int what, int64_t* out4);
+  void TimePredictKernel(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, int start_iteration,
+                         int num_iteration, int reps, float* mean_ms);
   std::string SaveModelToString(int start_iteration = 0, int num_iteration = -1) const;
   // GBDT::FeatureImportance (gbdt_model_text.cpp:638-674): importance_type 0 = number of splits, 1 = total gain
   std::vector<double> FeatureImportance(int num_iteration, int importance_type) const;
@@ -69,6 +83,9 @@ class Booster {
 
  private:
   void Boosting();  // gradients for the next tree (+ covariance-parameter fit when a GP model is attached)
+  gpbdev_ensemble_t DeviceEnsemble();  // the packed ensemble, brought up to date with models_
+  gpbdev_ensemble_t ensemble_ = nullptr;  // null: model-string booster in a process without a CUDA device (host walk)
+  size_t ensemble_trees_ = 0;             // number of trees of models_ the device ensemble holds
   struct ValidSet {
     const Dataset* data = nullptr;
     int64_t n = 0;

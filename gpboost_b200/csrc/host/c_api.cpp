@@ -351,14 +351,55 @@ int LGBM_BoosterGetEvalCounts(BoosterHandle handle, int* out_len) {
   API_END();
 }
 
+namespace {
+// C_API_PREDICT_* -> what of Booster::Predict (0 raw score: NORMAL and RAW_SCORE coincide for the L2 objective; 1 leaf index)
+int PredictWhat(int predict_type) {
+  if (predict_type == C_API_PREDICT_NORMAL || predict_type == C_API_PREDICT_RAW_SCORE) return 0;
+  if (predict_type == C_API_PREDICT_LEAF_INDEX) return 1;
+  if (predict_type == C_API_PREDICT_CONTRIB)
+    throw std::runtime_error("Feature contributions (pred_contrib, C_API_PREDICT_CONTRIB) are not supported by this build");
+  throw std::runtime_error("Unknown predict_type " + std::to_string(predict_type));
+}
+// number of values one prediction call writes (Booster::CalcNumPredict, c_api.cpp -> GBDT::NumPredictOneRow)
+int64_t NumPredictValues(gpb200::Booster* b, int64_t nrow, int what, int start_iteration, int num_iteration) {
+  if (what == 0) return nrow;
+  int first, count;
+  b->IterationRange(start_iteration, num_iteration, &first, &count);
+  return nrow * count;
+}
+}  // namespace
+
 int LGBM_BoosterPredictForMat(BoosterHandle handle, const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major,
                               int predict_type, int start_iteration, int num_iteration, const char* /*parameter*/,
                               int64_t* out_len, double* out_result) {
   API_BEGIN();
-  if (predict_type != C_API_PREDICT_NORMAL && predict_type != C_API_PREDICT_RAW_SCORE)
-    throw std::runtime_error("Only normal / raw-score prediction is supported by this build");
-  B(handle)->Predict(data, data_type, nrow, ncol, is_row_major, out_result, start_iteration, num_iteration);
-  *out_len = nrow;
+  const int what = PredictWhat(predict_type);
+  B(handle)->Predict(data, data_type, nrow, ncol, is_row_major, out_result, start_iteration, num_iteration, what);
+  *out_len = NumPredictValues(B(handle), nrow, what, start_iteration, num_iteration);
+  API_END();
+}
+
+int GPB200_BoosterPredictForMatHost(BoosterHandle handle, const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major,
+                                    int predict_type, int start_iteration, int num_iteration, const char* /*parameter*/,
+                                    int64_t* out_len, double* out_result) {
+  API_BEGIN();
+  const int what = PredictWhat(predict_type);
+  B(handle)->PredictHost(data, data_type, nrow, ncol, is_row_major, out_result, start_iteration, num_iteration, what);
+  *out_len = NumPredictValues(B(handle), nrow, what, start_iteration, num_iteration);
+  API_END();
+}
+
+int GPB200_BoosterPredictPlan(BoosterHandle handle, int data_type, int32_t ncol, int predict_type, int start_iteration, int num_iteration,
+                              int64_t* out4) {
+  API_BEGIN();
+  B(handle)->PredictPlan(data_type, ncol, start_iteration, num_iteration, PredictWhat(predict_type), out4);
+  API_END();
+}
+
+int GPB200_BoosterTimePredictKernel(BoosterHandle handle, const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major,
+                                    int start_iteration, int num_iteration, int reps, float* mean_ms) {
+  API_BEGIN();
+  B(handle)->TimePredictKernel(data, data_type, nrow, ncol, is_row_major, start_iteration, num_iteration, reps, mean_ms);
   API_END();
 }
 
@@ -477,11 +518,10 @@ int LGBM_BoosterGetNumFeature(BoosterHandle handle, int* out_len) {
   API_END();
 }
 
-int LGBM_BoosterCalcNumPredict(BoosterHandle handle, int num_row, int predict_type, int /*start_iteration*/, int /*num_iteration*/, int64_t* out_len) {
+int LGBM_BoosterCalcNumPredict(BoosterHandle handle, int num_row, int predict_type, int start_iteration, int num_iteration, int64_t* out_len) {
   API_BEGIN();
-  B(handle);
-  if (predict_type != 0 && predict_type != 1) throw std::runtime_error("Only normal and raw-score predictions are supported by the CUDA booster");
-  *out_len = num_row;  // one value per row (regression, one model per iteration)
+  // one value per row (regression, one model per iteration), or one leaf index per row and tree of the iteration range
+  *out_len = NumPredictValues(B(handle), num_row, PredictWhat(predict_type), start_iteration, num_iteration);
   API_END();
 }
 

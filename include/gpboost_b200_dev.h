@@ -363,6 +363,36 @@ GPBDEV_EXPORT int gpbdev_tree_sync(gpbdev_tree_t h);
 GPBDEV_EXPORT int64_t gpbdev_tree_launch_count(gpbdev_tree_t h);
 GPBDEV_EXPORT void* gpbdev_tree_stream(gpbdev_tree_t h);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Ensemble prediction on a raw feature matrix (csrc/dev/ensemble_predict.cu). Replaces the row loop of GBDT::PredictRaw /
+ * PredictLeafIndex (src/LightGBM/boosting/gbdt_prediction.cpp) over Tree::Predict / NumericalDecision (include/LightGBM/tree.h:329-347):
+ * numerical splits, all three missing types. Needs no learner: a prediction-only booster owns one as well. One stream per handle;
+ * every entry returns with that stream synchronised. No CPU fallback: gpbdev_ensemble_create fails without a CUDA device.
+ */
+typedef struct gpbdev_ensemble* gpbdev_ensemble_t;
+GPBDEV_EXPORT const char* gpbdev_ensemble_last_error(void);
+GPBDEV_EXPORT int gpbdev_ensemble_create(gpbdev_ensemble_t* out, int device);
+GPBDEV_EXPORT int gpbdev_ensemble_free(gpbdev_ensemble_t h);
+/* Install the trees (replaces the previous ones; kept packed in HBM until the next call). Tree k has leaf_offset[k+1] - leaf_offset[k]
+ * >= 1 leaves and one internal node less; per internal node (at node_offset[k] + i): split_feature (column of the matrix), threshold,
+ * decision_type (bit 1 default-left, bits 2-3 missing type; categorical bit 0 refused), left_child / right_child in the Tree
+ * convention (index of a LATER node of the same tree, or ~leaf). Child indices are checked, so every walk terminates. */
+GPBDEV_EXPORT int gpbdev_ensemble_set_trees(gpbdev_ensemble_t h, int num_trees, const int32_t* node_offset, const int32_t* leaf_offset,
+                                            const int32_t* split_feature, const double* threshold, const int8_t* decision_type,
+                                            const int32_t* left_child, const int32_t* right_child, const double* leaf_value);
+/* data_host: nrow x ncol in host memory, data_type 0 = float32 (widened to double first) / 1 = float64, row- or column-major. Trees
+ * [first_tree, first_tree + num_trees). what = 0: out_host[row] = 0.0 + leaf_first + ... in ensemble order, one fp64 add per tree
+ * (bitwise the host loop's result); what = 1: out_host[row * num_trees + k] = (double) leaf index of the row in tree first_tree + k. */
+GPBDEV_EXPORT int gpbdev_ensemble_predict(gpbdev_ensemble_t h, const void* data_host, int data_type, int64_t nrow, int ncol, int is_row_major,
+                                          int first_tree, int num_trees, int what, double* out_host);
+/* How gpbdev_ensemble_predict would run this shape: out4 = { rows of a block's tile, rows of one staging chunk, 1 when the tile's
+ * features are staged in shared memory (0: read from global memory), number of shared-memory stages the tree range is split into } */
+GPBDEV_EXPORT int gpbdev_ensemble_plan(gpbdev_ensemble_t h, int data_type, int ncol, int first_tree, int num_trees, int what, int64_t* out4);
+/* bench hook: the whole matrix is copied to the device once, then mean device time (CUDA events) of `reps` launches of the what = 0
+ * kernel over all nrow rows; algorithmic bytes per launch nrow * ncol * sizeof(element) + nrow * 8 */
+GPBDEV_EXPORT int gpbdev_ensemble_time_kernel(gpbdev_ensemble_t h, const void* data_host, int data_type, int64_t nrow, int ncol,
+                                              int is_row_major, int first_tree, int num_trees, int reps, float* mean_ms);
+
 #ifdef __cplusplus
 }
 #endif
