@@ -106,7 +106,10 @@ template <int COV, int MODE, int DIM>
 FactorKernel pick_cap(int m) {
   if (m <= 10) return gpb::vecchia_factor_kernel<COV, MODE, DIM, 10>;
   if (m <= 20) return gpb::vecchia_factor_kernel<COV, MODE, DIM, 20>;
-  return gpb::vecchia_factor_kernel<COV, MODE, DIM, 30>;
+  // d = 2, 20 < m <= 30: NLL / STORE / GRAD run the two-observation kernel (vecchia_nll2.cuh), so only the factor-derivative
+  // modes are instantiated at this cap
+  if constexpr (DIM == 2 && MODE != gpb::MODE_STORE_GRAD && MODE != gpb::MODE_STORE_GRAD2) return nullptr;
+  else return gpb::vecchia_factor_kernel<COV, MODE, DIM, 30>;
 }
 template <int COV, int MODE>
 FactorKernel pick_dim(int d, int m) {
@@ -195,9 +198,6 @@ struct gpbdev_vecchia {
   bool stored_latent = false, last_latent = false;
   double stored_var = 0., stored_range = 0., last_var = 0., last_range = 0.;
   int knn_replayed = 0;  // queries whose neighbour set was re-derived by the exact replay of the reference walk
-  // kernel switches, read from the environment when the engine is created (gpbdev_vecchia_create)
-  bool grad_stores = true;  // GPB200_GRAD_STORES=0: no STORE shortcut after a gradient pass, no extra stores in that pass
-  bool nll1_only = false;   // GPB200_NLL_KERNEL=1: one-observation kernel also at d = 2, 20 < m <= 30
   std::vector<int32_t> nn_host;  // kept for the lazy CSC build
   // linear regression covariates (covariates.cuh), lazy
   int p = 0;                       // number of covariates
@@ -262,9 +262,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
   CUDA_TRY(cudaSetDevice(h->device));
   // GPBoost iteration: OptimCovPar's last accepted trial was a gradient pass at the final parameters on this response, and
   // CalcGradient asks for the factor at the same state right after (regression_objective.hpp:164-165): nothing to recompute.
-  // GPB200_GRAD_STORES=0 switches the shortcut (and the extra stores of the gradient pass) off.
-  const bool grad_stores = h->grad_stores;
-  if (mode == gpb::MODE_STORE && !latent && grad_stores && h->factor_stored && h->stored_cov == cov_type && h->stored_latent == latent &&
+  if (mode == gpb::MODE_STORE && !latent && h->factor_stored && h->stored_cov == cov_type && h->stored_latent == latent &&
       h->stored_var == var && h->stored_range == range && h->last_cov == cov_type && h->last_latent == latent && h->last_var == var &&
       h->last_range == range)
     return 0;
@@ -282,7 +280,6 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
   gpb::FactorArgs a;
   a.coords = h->coords; a.nn = h->nn; a.y = h->y;
   a.A = h->A; a.Dinv = h->Dinv; a.w = h->u;
-  if (mode == gpb::MODE_GRAD && !grad_stores) a.A = nullptr;  // (only the two-observation gradient pass looks at it)
   a.partials = h->partials;
   a.n = h->n; a.row_begin = h->row_begin; a.row_end = h->row_end;
   a.m = h->m; a.d = h->d; a.var = var; a.range = range;
@@ -293,6 +290,19 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
     CUDA_TRY(cudaMemcpyToSymbolAsync(gpb::g_factor_dD, &h->dD, sizeof(double*), 0, cudaMemcpyHostToDevice, h->stream));
   }
   if (latent && mode == gpb::MODE_GRAD) return fail("gpbdev_vecchia_eval: the gradient pass assumes a Gaussian likelihood");
+  // every pass ends alike: the fixed-order reduction of its `rows` per-warp partial rows into the sums, on row shards the
+  // all-reduce of the sums over the ranks on this stream (NCCL kernel), and the record of a stored factor
+  auto finish = [&](int64_t rows) -> int {
+    CUDA_TRY(cudaGetLastError());
+    reduce_partials_kernel<<<1, 256, 0, h->stream>>>(h->partials, rows, h->sums);
+    CUDA_TRY(cudaGetLastError());
+    h->launches += 2;
+    if (h->allreduce && !latent) {
+      if (h->allreduce(h->allreduce_ctx, h->sums, gpb::kNumAcc, (void*)h->stream)) return fail("gpbdev_vecchia_eval: device all-reduce failed");
+    }
+    if (mode == gpb::MODE_STORE || mode == gpb::MODE_STORE_GRAD) h->factor_stored = true;
+    return 0;
+  };
   if (h->m > gpb::kMaxNeighbors) {  // 30 < num_neighbors <= 60: shared-memory kernel (vecchia_big.cuh), same sums and factor layout
     if (mode == gpb::MODE_STORE_GRAD) return fail("gpbdev_vecchia_eval: the factor derivative (non-Gaussian likelihoods) supports num_neighbors <= 30");
     gpb::BigArgs b;
@@ -308,19 +318,10 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
     int grid = std::min(h->num_sms, (int)((h->grid_cap * gpb::kWarpsPerBlock) / warps));  // one CTA per SM; partials has grid_cap * 4 rows
     grid = std::max(grid, 1);
     bk<<<grid, warps * 32, bsmem, h->stream>>>(b);
-    CUDA_TRY(cudaGetLastError());
-    reduce_partials_kernel<<<1, 256, 0, h->stream>>>(h->partials, (int64_t)grid * warps, h->sums);
-    CUDA_TRY(cudaGetLastError());
-    h->launches += 2;
-    if (h->allreduce && !latent) {
-      if (h->allreduce(h->allreduce_ctx, h->sums, gpb::kNumAcc, (void*)h->stream)) return fail("gpbdev_vecchia_eval: device all-reduce failed");
-    }
-    if (mode == gpb::MODE_STORE) h->factor_stored = true;
-    return 0;
+    return finish((int64_t)grid * warps);
   }
-  // likelihood and gradient passes at the headline shape (d = 2, 20 < m <= 30): two observations per warp (vecchia_nll2.cuh);
-  // GPB200_NLL_KERNEL=1 keeps the one-observation kernel
-  if ((mode == gpb::MODE_NLL || mode == gpb::MODE_STORE || (mode == gpb::MODE_GRAD && !latent)) && h->d == 2 && h->m > 20 && !h->nll1_only) {
+  // likelihood and gradient passes at the headline shape (d = 2, 20 < m <= 30): two observations per warp (vecchia_nll2.cuh)
+  if ((mode == gpb::MODE_NLL || mode == gpb::MODE_STORE || (mode == gpb::MODE_GRAD && !latent)) && h->d == 2 && h->m > 20) {
     FactorKernel k2 = nullptr;
 #define GPB_PICK2(COVID)                                                                                                              \
     k2 = mode == gpb::MODE_NLL ? gpb::vecchia_nll2_kernel<COVID, gpb::MODE_NLL>                                                      \
@@ -340,14 +341,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
     int grid2 = std::max(per_sm2, 1) * h->num_sms;
     grid2 = std::max(1, std::min(grid2, h->grid_cap / 2));  // two partial rows per warp
     k2<<<grid2, gpb::kWarpsPerBlock * 32, smem2, h->stream>>>(a);
-    CUDA_TRY(cudaGetLastError());
-    reduce_partials_kernel<<<1, 256, 0, h->stream>>>(h->partials, (int64_t)grid2 * gpb::kWarpsPerBlock * 2, h->sums);
-    CUDA_TRY(cudaGetLastError());
-    h->launches += 2;
-    if (h->allreduce && !latent) {
-      if (h->allreduce(h->allreduce_ctx, h->sums, gpb::kNumAcc, (void*)h->stream)) return fail("gpbdev_vecchia_eval: device all-reduce failed");
-    }
-    if (mode == gpb::MODE_STORE) h->factor_stored = true;
+    if (finish((int64_t)grid2 * gpb::kWarpsPerBlock * 2)) return -1;
     if (mode == gpb::MODE_GRAD && a.A != nullptr) {  // the pass also wrote A, D^-1, u (vecchia_nll2_kernel<GRAD>)
       h->factor_stored = true;
       h->stored_cov = cov_type; h->stored_latent = false; h->stored_var = var; h->stored_range = range;
@@ -355,6 +349,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
     return 0;
   }
   FactorKernel k = pick_kernel(cov_type, mode, h->d, h->m);
+  if (!k) return fail("gpbdev_vecchia_eval: no one-observation factor kernel for this mode at d = 2, num_neighbors > 20");
   const size_t smem = sizeof(double) * gpb::kWarpsPerBlock * (32 * gpb::kLd + 32 * h->d + 64);
   CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -364,15 +359,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
   int grid = std::max(per_sm, 1) * h->num_sms;
   if (grid > h->grid_cap) grid = h->grid_cap;
   k<<<grid, gpb::kWarpsPerBlock * 32, smem, h->stream>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  reduce_partials_kernel<<<1, 256, 0, h->stream>>>(h->partials, (int64_t)grid * gpb::kWarpsPerBlock, h->sums);
-  CUDA_TRY(cudaGetLastError());
-  h->launches += 2;
-  if (h->allreduce && !latent) {  // row shards: the 9 sums are summed over the ranks on this stream (NCCL kernel)
-    if (h->allreduce(h->allreduce_ctx, h->sums, gpb::kNumAcc, (void*)h->stream)) return fail("gpbdev_vecchia_eval: device all-reduce failed");
-  }
-  if (mode == gpb::MODE_STORE || mode == gpb::MODE_STORE_GRAD) h->factor_stored = true;
-  return 0;
+  return finish((int64_t)grid * gpb::kWarpsPerBlock);
 }
 
 }  // namespace
@@ -424,8 +411,6 @@ int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, i
   CUDA_TRY(cudaSetDevice(device));
   gpbdev_vecchia* h = new gpbdev_vecchia();
   h->device = device; h->n = n; h->d = d; h->m = m; h->row_begin = row_begin; h->row_end = row_end;
-  if (const char* e = std::getenv("GPB200_GRAD_STORES")) h->grad_stores = std::string(e) != "0";
-  if (const char* e = std::getenv("GPB200_NLL_KERNEL")) h->nll1_only = std::string(e) == "1";
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   h->num_sms = prop.multiProcessorCount;

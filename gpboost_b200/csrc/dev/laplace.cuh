@@ -28,16 +28,13 @@
 // + 8 written, plus 12m for the pattern and A, amortised over the t columns.
 #include <cooperative_groups.h>
 
-#include <chrono>
-#include <cstdlib>
-
 namespace gpl {
 
 constexpr unsigned long long kSentinel = 0x7ff8dead0badf00dULL;  // quiet-NaN payload no computation produces
 constexpr int kMaxCols = 128;
 constexpr int kBlock = 256;
 constexpr int kSpinLimit = 1 << 22;
-__device__ int g_sleep_ns = 100;  // back-off between polls of a dependency that is still in flight
+constexpr int kSleepNs = 100;  // back-off between polls of a dependency that is still in flight
 
 struct Coef { double v[kMaxCols]; };
 
@@ -61,7 +58,7 @@ __device__ __forceinline__ double poll(const double* p, int* err) {
   int spins = 0;
   while (is_sent(v)) {
     if (++spins > kSpinLimit) { atomicExch(err, 1); return 0.; }
-    __nanosleep(g_sleep_ns);
+    __nanosleep(kSleepNs);
     v = ld_gpu(p);
   }
   return v;
@@ -299,7 +296,7 @@ __device__ __forceinline__ void resolve_deps(double (&v)[N], const double* base,
         if (((ready >> k) & 1u) && __any_sync(0xffffffffu, is_sent(v[k]))) still |= 1u << k;  // row only partly visible yet
     } else {
       if (++spins > kSpinLimit) { if (lane == 0) atomicExch(err, 1); return; }
-      __nanosleep(g_sleep_ns);
+      __nanosleep(kSleepNs);
     }
     pend = still;
   }
@@ -435,160 +432,6 @@ __global__ void csc_gather_kernel(const double* __restrict__ A, const int32_t* _
     A_csc[e] = A[pos];
     csc_row[e] = pos / m;
   }
-}
-
-// ---- tiled operator kernels (opt-in, see lap_build_tiles): neighbour blocks staged in shared memory by bulk async copies ---
-// mv_B / mv_Bt gather m + 1 rows of the multi-vector per row of B: at t = 50 that is 12.4 KB through L2 per row although rows that
-// are close in space share most of their neighbours. Here 32 rows that are consecutive on the Morton curve form a TILE; the
-// distinct source rows of a tile (~205 of 992 gathers at n = 1e6, m = 30; the lists are a static property of the pattern, built
-// once) are brought into shared memory ONCE, each by one cp.async.bulk (TMA bulk engine, 8 t contiguous bytes) signalling an
-// mbarrier with complete_tx, and the 32 x (m + 1) products are taken from shared memory (lane = column: conflict-free). Two
-// CTAs per SM alternate between their load and compute phases. L2 -> SM traffic drops from (m + 1) rows per row to ~6.4.
-// Sources beyond the tile's capacity (early points with far neighbours; rare) are marked in the slot table and read from global.
-constexpr int kTileRows = 32;
-constexpr int kTileCap = 272;          // source rows held per tile: 272 * 400 B = 108.8 KB at t = 50 -> two CTAs per SM
-constexpr int kTileThreads = 128;
-constexpr uint16_t kSlotNone = 0xFFFF;  // padded neighbour slot
-constexpr uint16_t kSlotGlobal = 0xFFFE;  // source did not fit the tile: read from global memory
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count));
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* b) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src),
-               "r"(bytes), "r"(smem_u32(b))
-               : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* b, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-               : "=r"(ok)
-               : "r"(smem_u32(b)), "r"(parity)
-               : "memory");
-  return ok != 0;
-}
-
-// T[i,:] = s_i (X[i,:] - sum_k A[i,k] X[nn[i,k],:]) for the rows of tile `tile` (positions 32 tile .. of `order`)
-// tile_ptr / tile_src: sources of each tile; slot[p * (m + 1) + 0] = slot of the row itself, + 1 + k = slot of neighbour k
-__global__ void __launch_bounds__(kTileThreads) mv_B_tiled_kernel(const double* __restrict__ A, const int32_t* __restrict__ nn, int m, int64_t n, int t,
-                                                                 const double* __restrict__ Dinv, const double* __restrict__ X, double* __restrict__ T,
-                                                                 const int32_t* __restrict__ order, int ntiles, const int32_t* __restrict__ tile_ptr,
-                                                                 const int32_t* __restrict__ tile_src, const uint16_t* __restrict__ slot) {
-  extern __shared__ __align__(128) double tbuf[];
-  __shared__ __align__(8) uint64_t bar;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const uint32_t row_bytes = (uint32_t)t * 8u;
-  if (tid == 0) mbar_init(&bar, 1);
-  __syncthreads();
-  uint32_t parity = 0;
-  const int c0 = lane, c1 = 32 + lane;
-  const bool on0 = c0 < t, on1 = c1 < t;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int s0 = tile_ptr[tile];
-    const int nd = min(tile_ptr[tile + 1] - s0, kTileCap);
-    if (tid == 0) mbar_expect_tx(&bar, (uint32_t)nd * row_bytes);
-    for (int k = tid; k < nd; k += kTileThreads) bulk_g2s(tbuf + (size_t)k * t, X + (size_t)tile_src[s0 + k] * t, row_bytes, &bar);
-    // the rows' own data while the copies fly
-    const int64_t pbase = (int64_t)tile * kTileRows + w * (kTileRows / 4);
-    while (!mbar_try_wait(&bar, parity)) {}
-    parity ^= 1u;
-    for (int r = 0; r < kTileRows / 4; ++r) {
-      const int64_t p = pbase + r;
-      if (p >= n) break;
-      const int64_t i = order[p];
-      const uint16_t sl = lane <= m ? slot[p * (m + 1) + lane] : kSlotNone;   // lane 0: own row, lane 1 + k: neighbour k
-      const double ak = (lane >= 1 && lane <= m && sl != kSlotNone) ? A[i * m + lane - 1] : 0.;
-      const int32_t jn = (lane >= 1 && lane <= m) ? nn[i * m + lane - 1] : -1;
-      const unsigned s_self = __shfl_sync(0xffffffffu, (unsigned)sl, 0);
-      double acc0 = 0., acc1 = 0.;
-      if (s_self == kSlotGlobal) { if (on0) acc0 = X[i * t + c0]; if (on1) acc1 = X[i * t + c1]; }
-      else { if (on0) acc0 = tbuf[(size_t)s_self * t + c0]; if (on1) acc1 = tbuf[(size_t)s_self * t + c1]; }
-      for (int k = 1; k <= m; ++k) {
-        const unsigned sk = __shfl_sync(0xffffffffu, (unsigned)sl, k);
-        const double a = __shfl_sync(0xffffffffu, ak, k);
-        const int32_t j = __shfl_sync(0xffffffffu, jn, k);
-        if (sk == kSlotNone) continue;
-        if (sk == kSlotGlobal) {
-          if (on0) acc0 -= a * X[(int64_t)j * t + c0];
-          if (on1) acc1 -= a * X[(int64_t)j * t + c1];
-        } else {
-          if (on0) acc0 -= a * tbuf[(size_t)sk * t + c0];
-          if (on1) acc1 -= a * tbuf[(size_t)sk * t + c1];
-        }
-      }
-      const double s = Dinv ? Dinv[i] : 1.;
-      if (on0) T[i * t + c0] = s * acc0;
-      if (on1) T[i * t + c1] = s * acc1;
-    }
-    __syncthreads();  // every warp is done with the buffer before the next tile's copies land in it
-  }
-}
-
-// V[j,:] = T[j,:] - sum_{e in column j} A_csc[e] T[row_e,:] + W[j] X[j,:];  per-warp partial dots X[j,c] V[j,c] (columns c, 32 + c)
-// slot_e[e]: slot of the source row of CSC entry e within the tile of its column
-__global__ void __launch_bounds__(kTileThreads) mv_Bt_tiled_kernel(const double* __restrict__ A_csc, const int32_t* __restrict__ colptr,
-                                                                  const int32_t* __restrict__ csc_row, int64_t n, int t,
-                                                                  const double* __restrict__ T, const double* __restrict__ W,
-                                                                  const double* __restrict__ X, double* __restrict__ V, double* __restrict__ partial,
-                                                                  const int32_t* __restrict__ order, int ntiles, const int32_t* __restrict__ tile_ptr,
-                                                                  const int32_t* __restrict__ tile_src, const uint16_t* __restrict__ slot_e) {
-  extern __shared__ __align__(128) double tbuf[];
-  __shared__ __align__(8) uint64_t bar;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const uint32_t row_bytes = (uint32_t)t * 8u;
-  if (tid == 0) mbar_init(&bar, 1);
-  __syncthreads();
-  uint32_t parity = 0;
-  const int c0 = lane, c1 = 32 + lane;
-  const bool on0 = c0 < t, on1 = c1 < t;
-  double dot0 = 0., dot1 = 0.;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int s0 = tile_ptr[tile];
-    const int nd = min(tile_ptr[tile + 1] - s0, kTileCap);
-    if (tid == 0) mbar_expect_tx(&bar, (uint32_t)nd * row_bytes);
-    for (int k = tid; k < nd; k += kTileThreads) bulk_g2s(tbuf + (size_t)k * t, T + (size_t)tile_src[s0 + k] * t, row_bytes, &bar);
-    const int64_t pbase = (int64_t)tile * kTileRows + w * (kTileRows / 4);
-    while (!mbar_try_wait(&bar, parity)) {}
-    parity ^= 1u;
-    for (int r = 0; r < kTileRows / 4; ++r) {
-      const int64_t p = pbase + r;
-      if (p >= n) break;
-      const int64_t j = order[p];
-      double acc0 = on0 ? T[j * t + c0] : 0., acc1 = on1 ? T[j * t + c1] : 0.;
-      const int e0 = colptr[j], e1 = colptr[j + 1];
-      for (int eb = e0; eb < e1; eb += 32) {
-        const int e = eb + lane;
-        const unsigned sl = e < e1 ? (unsigned)slot_e[e] : (unsigned)kSlotNone;
-        const double ae = e < e1 ? A_csc[e] : 0.;
-        const int32_t re = e < e1 ? csc_row[e] : 0;
-        const int cnt = min(32, e1 - eb);
-        for (int q = 0; q < cnt; ++q) {
-          const unsigned sk = __shfl_sync(0xffffffffu, sl, q);
-          const double a = __shfl_sync(0xffffffffu, ae, q);
-          const int32_t row = __shfl_sync(0xffffffffu, re, q);
-          if (sk == kSlotGlobal) {
-            if (on0) acc0 -= a * T[(int64_t)row * t + c0];
-            if (on1) acc1 -= a * T[(int64_t)row * t + c1];
-          } else {
-            if (on0) acc0 -= a * tbuf[(size_t)sk * t + c0];
-            if (on1) acc1 -= a * tbuf[(size_t)sk * t + c1];
-          }
-        }
-      }
-      const double wj = W ? W[j] : 0.;
-      if (on0) { const double xj = X[j * t + c0]; const double v = acc0 + wj * xj; V[j * t + c0] = v; dot0 += xj * v; }
-      if (on1) { const double xj = X[j * t + c1]; const double v = acc1 + wj * xj; V[j * t + c1] = v; dot1 += xj * v; }
-    }
-    __syncthreads();
-  }
-  const size_t gw = (size_t)blockIdx.x * (kTileThreads / 32) + w;
-  if (on0) partial[gw * kMaxCols + c0] = dot0;
-  if (on1) partial[gw * kMaxCols + c1] = dot1;
 }
 
 // ---- likelihood pieces: the three per-row kernels (prep_kernel, row_stats_kernel, grad_coef_kernel) are templated on
@@ -873,10 +716,6 @@ struct gpb_laplace_state {
   int grid = 0;           // persistent cooperative grid (blocks): what is co-resident for the polling kernels
   int grid_mv = 0;        // grid of the ordinary (non-polling) row kernels
   int grid_v = 0;         // cooperative grid of the single-vector polling kernels (few registers: more resident warps)
-  // tiles of 32 Morton-consecutive rows with their distinct source rows (tiled operator kernels; built once per model, lazily)
-  int ntiles = 0, tiled = -1;      // tiled: -1 not decided, 0 off (GPB200_LAPLACE_TILED=0, no Morton order, ...), 1 on
-  int32_t *tb_ptr = nullptr, *tb_src = nullptr, *tt_ptr = nullptr, *tt_src = nullptr;
-  uint16_t *tb_slot = nullptr, *tt_slot = nullptr;
   int32_t* order = nullptr;  // n: processing order of the order-free row kernels (Morton order of the locations); null = by index
   int nwarps = 0;
   double *mode = nullptr, *mode_new = nullptr, *upd = nullptr, *dir = nullptr, *rhs = nullptr, *W = nullptr, *dw = nullptr, *fe = nullptr;
@@ -907,7 +746,6 @@ void laplace_release(gpbdev_vecchia* h) {
   for (double* b : bufs) cudaFree(b);
   cudaFree(L->err);
   cudaFree(L->order);
-  cudaFree(L->tb_ptr); cudaFree(L->tb_src); cudaFree(L->tt_ptr); cudaFree(L->tt_src); cudaFree(L->tb_slot); cudaFree(L->tt_slot);
   cudaFreeHost(L->colsum_host);
   cudaFreeHost(L->stage);
   delete L;
@@ -936,10 +774,6 @@ int laplace_ensure(gpbdev_vecchia* h) {
   CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_v, gpl::v_trs_bwd_kernel, gpl::kBlock, 0));
   CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_v2, gpl::v_trs_fwd_kernel, gpl::kBlock, 0));
   L->grid_v = std::max(1, std::min(std::min(per_v, per_v2), 4)) * h->num_sms;
-  if (const char* e = std::getenv("GPB200_TRS_SLEEP_NS")) {
-    const int ns = std::max(0, std::atoi(e));
-    CUDA_TRY(cudaMemcpyToSymbol(gpl::g_sleep_ns, &ns, sizeof(int)));
-  }
   L->nwarps = std::max(std::max(L->grid, L->grid_mv), L->grid_v) * (gpl::kBlock / 32) + 1;
   double** vecs[] = {&L->mode, &L->mode_new, &L->upd, &L->dir, &L->rhs, &L->W, &L->dw, &L->fe, &L->r, &L->z, &L->hv, &L->v, &L->tt, &L->yy};
   for (double** p : vecs) {
@@ -953,9 +787,9 @@ int laplace_ensure(gpbdev_vecchia* h) {
   CUDA_TRY(cudaMalloc(&L->err, sizeof(int)));
   CUDA_TRY(cudaMemsetAsync(L->err, 0, sizeof(int), h->stream));
   CUDA_TRY(cudaMallocHost(&L->stage, sizeof(double) * n));
-  // processing order of mv_B / mv_Bt: Morton (Z-order) curve over the bounding box of the locations (d = 2: 2 x 16 bits, d = 3: 3 x 10 bits)
-  const char* oe = std::getenv("GPB200_LAPLACE_ORDER");
-  if ((h->d == 2 || h->d == 3) && !(oe && std::string(oe) == "index")) {
+  // processing order of mv_B / mv_Bt: Morton (Z-order) curve over the bounding box of the locations (d = 2: 2 x 16 bits, d = 3: 3 x 10 bits),
+  // index order at every other d
+  if (h->d == 2 || h->d == 3) {
     const int d = h->d;
     std::vector<double> c((size_t)n * d);
     CUDA_TRY(cudaMemcpy(c.data(), h->coords, sizeof(double) * n * d, cudaMemcpyDeviceToHost));
@@ -1008,19 +842,6 @@ int coop_launch(gpbdev_vecchia* h, int grid, K kernel, Args... args) {
 inline int lap_groups(int t) { return (t + 31) / 32; }
 inline int lap_grid(int grid, int G) { return std::max(G, grid - grid % G); }
 
-// phase timers (GPB200_LAPLACE_TRACE=1 prints them): every timed helper ends with a stream synchronisation
-struct LapTrace {
-  bool on = std::getenv("GPB200_LAPLACE_TRACE") != nullptr;
-  double t[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  int c[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-};
-LapTrace g_trace;
-struct LapScope {
-  int id; std::chrono::steady_clock::time_point t0;
-  explicit LapScope(int i) : id(i), t0(std::chrono::steady_clock::now()) {}
-  ~LapScope() { g_trace.t[id] += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); ++g_trace.c[id]; }
-};
-
 // Coefficients in CSC order: the B^T products and the backward solves walk columns, and A[csc_pos[e]] is a random 8-byte read
 // (one 32-byte sector each) where A_csc[e] streams. Rebuilt after every latent factorisation (one gather over nnz entries).
 int lap_refresh_csc_coefs(gpbdev_vecchia* h) {
@@ -1039,137 +860,21 @@ int lap_refresh_csc_coefs(gpbdev_vecchia* h) {
   return 0;
 }
 
-// Builds the tile lists of the tiled operator kernels (once per model; the pattern is static): for every tile of 32 Morton-consecutive
-// rows the sorted distinct source rows of B (the rows and their neighbours) and of B^T (the columns' dependents), and for every
-// (row, neighbour) / CSC entry the slot of its source inside the tile (or kSlotGlobal beyond the tile's capacity).
-int lap_build_tiles(gpbdev_vecchia* h) {
-  gpb_laplace_state* L = h->lap;
-  if (L->tiled >= 0) return 0;
-  L->tiled = 0;
-  // opt-in (GPB200_LAPLACE_TILED=1): the staged kernels lost to the plain gather kernels in Morton order at n = 1e6, t = 50
-  // (not re-measured on H100): ~200 bulk copies of 400
-  // bytes per tile cost more than they save while two 4-warp CTAs per SM cannot match the gather kernels' memory-level parallelism
-  const char* te = std::getenv("GPB200_LAPLACE_TILED");
-  if (!L->order || !(te && std::string(te) == "1") || h->m > 30) return 0;
-  const int64_t n = h->n;
-  const int m = h->m;
-  std::vector<int32_t> ord((size_t)n);
-  CUDA_TRY(cudaMemcpy(ord.data(), L->order, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
-  if (h->nn_host.empty()) {
-    h->nn_host.resize((size_t)n * m);
-    CUDA_TRY(cudaMemcpy(h->nn_host.data(), h->nn, sizeof(int32_t) * n * m, cudaMemcpyDeviceToHost));
-  }
-  const std::vector<int32_t>& nnh = h->nn_host;
-  std::vector<int32_t> colptr((size_t)n + 1), crow;
-  CUDA_TRY(cudaMemcpy(colptr.data(), h->colptr, sizeof(int32_t) * (n + 1), cudaMemcpyDeviceToHost));
-  crow.resize((size_t)colptr[n]);
-  {
-    std::vector<int32_t> pos((size_t)colptr[n]);
-    CUDA_TRY(cudaMemcpy(pos.data(), h->csc_pos, sizeof(int32_t) * pos.size(), cudaMemcpyDeviceToHost));
-    for (size_t e = 0; e < pos.size(); ++e) crow[e] = pos[e] / m;
-  }
-  const int ntiles = (int)((n + gpl::kTileRows - 1) / gpl::kTileRows);
-  std::vector<std::vector<int32_t>> srcB((size_t)ntiles), srcT((size_t)ntiles);
-  std::vector<uint16_t> slotB((size_t)n * (m + 1), gpl::kSlotNone), slotT((size_t)colptr[n], gpl::kSlotNone);
-#pragma omp parallel for schedule(dynamic, 64)
-  for (int tl = 0; tl < ntiles; ++tl) {
-    const int64_t p0 = (int64_t)tl * gpl::kTileRows, p1 = std::min<int64_t>(p0 + gpl::kTileRows, n);
-    auto slot_of = [](const std::vector<int32_t>& u, int32_t id) -> uint16_t {
-      const int k = (int)(std::lower_bound(u.begin(), u.end(), id) - u.begin());
-      return k < gpl::kTileCap ? (uint16_t)k : gpl::kSlotGlobal;
-    };
-    {  // B: rows + neighbours
-      std::vector<int32_t>& u = srcB[(size_t)tl];
-      for (int64_t p = p0; p < p1; ++p) {
-        const int32_t i = ord[(size_t)p];
-        u.push_back(i);
-        for (int k = 0; k < m; ++k) { const int32_t j = nnh[(size_t)i * m + k]; if (j >= 0) u.push_back(j); }
-      }
-      std::sort(u.begin(), u.end());
-      u.erase(std::unique(u.begin(), u.end()), u.end());
-      for (int64_t p = p0; p < p1; ++p) {
-        const int32_t i = ord[(size_t)p];
-        slotB[(size_t)p * (m + 1)] = slot_of(u, i);
-        for (int k = 0; k < m; ++k) { const int32_t j = nnh[(size_t)i * m + k]; if (j >= 0) slotB[(size_t)p * (m + 1) + 1 + k] = slot_of(u, j); }
-      }
-      if ((int)u.size() > gpl::kTileCap) u.resize(gpl::kTileCap);
-    }
-    {  // B^T: the dependents of the tile's columns
-      std::vector<int32_t>& u = srcT[(size_t)tl];
-      for (int64_t p = p0; p < p1; ++p) {
-        const int32_t j = ord[(size_t)p];
-        for (int32_t e = colptr[(size_t)j]; e < colptr[(size_t)j + 1]; ++e) u.push_back(crow[(size_t)e]);
-      }
-      std::sort(u.begin(), u.end());
-      u.erase(std::unique(u.begin(), u.end()), u.end());
-      for (int64_t p = p0; p < p1; ++p) {
-        const int32_t j = ord[(size_t)p];
-        for (int32_t e = colptr[(size_t)j]; e < colptr[(size_t)j + 1]; ++e) slotT[(size_t)e] = slot_of(u, crow[(size_t)e]);
-      }
-      if ((int)u.size() > gpl::kTileCap) u.resize(gpl::kTileCap);
-    }
-  }
-  std::vector<int32_t> pb((size_t)ntiles + 1, 0), pt((size_t)ntiles + 1, 0);
-  for (int tl = 0; tl < ntiles; ++tl) { pb[(size_t)tl + 1] = pb[(size_t)tl] + (int32_t)srcB[(size_t)tl].size(); pt[(size_t)tl + 1] = pt[(size_t)tl] + (int32_t)srcT[(size_t)tl].size(); }
-  std::vector<int32_t> fb((size_t)pb[(size_t)ntiles]), ft((size_t)std::max(pt[(size_t)ntiles], 1));
-  for (int tl = 0; tl < ntiles; ++tl) {
-    std::copy(srcB[(size_t)tl].begin(), srcB[(size_t)tl].end(), fb.begin() + pb[(size_t)tl]);
-    std::copy(srcT[(size_t)tl].begin(), srcT[(size_t)tl].end(), ft.begin() + pt[(size_t)tl]);
-  }
-  auto up = [&](void** dst, const void* src, size_t bytes) -> cudaError_t {
-    cudaError_t e = cudaMalloc(dst, std::max<size_t>(bytes, 16));
-    if (e == cudaSuccess) e = cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
-    return e;
-  };
-  CUDA_TRY(up((void**)&L->tb_ptr, pb.data(), sizeof(int32_t) * pb.size()));
-  CUDA_TRY(up((void**)&L->tt_ptr, pt.data(), sizeof(int32_t) * pt.size()));
-  CUDA_TRY(up((void**)&L->tb_src, fb.data(), sizeof(int32_t) * fb.size()));
-  CUDA_TRY(up((void**)&L->tt_src, ft.data(), sizeof(int32_t) * (size_t)pt[(size_t)ntiles]));
-  CUDA_TRY(up((void**)&L->tb_slot, slotB.data(), sizeof(uint16_t) * slotB.size()));
-  CUDA_TRY(up((void**)&L->tt_slot, slotT.data(), sizeof(uint16_t) * slotT.size()));
-  const int max_smem = (int)(sizeof(double) * gpl::kTileCap * 64);
-  CUDA_TRY(cudaFuncSetAttribute(gpl::mv_B_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-  CUDA_TRY(cudaFuncSetAttribute(gpl::mv_Bt_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-  L->ntiles = ntiles;
-  L->tiled = 1;
-  return 0;
-}
-
-// multi-vector products with B and B^T: tiled kernels (bulk-copy staging) when the tile lists exist and the rows are 16-byte
-// multiples, the gather kernels otherwise. *prow = rows of the per-warp partial dots the B^T product leaves behind.
-inline bool lap_use_tiles(gpbdev_vecchia* h, int t) {
-  gpb_laplace_state* L = h->lap;
-  return L->tiled == 1 && t > 1 && (t % 2) == 0 && t <= 64;
-}
+// multi-vector products with B and B^T: gather kernels over G = ceil(t / 32) column groups, rows in the engine's order.
+// *prow = rows of the per-warp partial dots the B^T product leaves behind.
 int lap_mv_B(gpbdev_vecchia* h, int t, const double* Dinv, const double* X, double* T) {
   gpb_laplace_state* L = h->lap;
-  if (L->tiled < 0 && lap_build_tiles(h)) return -1;
-  if (lap_use_tiles(h, t)) {
-    const size_t smem = sizeof(double) * (size_t)gpl::kTileCap * t;
-    const int grid = std::min(L->ntiles, 2 * h->num_sms);
-    gpl::mv_B_tiled_kernel<<<grid, gpl::kTileThreads, smem, h->stream>>>(h->A, h->nn, h->m, h->n, t, Dinv, X, T, L->order, L->ntiles, L->tb_ptr, L->tb_src, L->tb_slot);
-  } else {
-    const int G = lap_groups(t), grid = lap_grid(L->grid_mv, G);
-    gpl::mv_B_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->A, h->nn, h->m, h->n, t, G, Dinv, X, T, L->order);
-  }
+  const int G = lap_groups(t), grid = lap_grid(L->grid_mv, G);
+  gpl::mv_B_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->A, h->nn, h->m, h->n, t, G, Dinv, X, T, L->order);
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
   return 0;
 }
 int lap_mv_Bt(gpbdev_vecchia* h, int t, const double* Tin, const double* W, const double* X, double* V, int* prow) {
   gpb_laplace_state* L = h->lap;
-  if (L->tiled < 0 && lap_build_tiles(h)) return -1;
-  if (lap_use_tiles(h, t)) {
-    const size_t smem = sizeof(double) * (size_t)gpl::kTileCap * t;
-    const int grid = std::min(L->ntiles, 2 * h->num_sms);
-    gpl::mv_Bt_tiled_kernel<<<grid, gpl::kTileThreads, smem, h->stream>>>(h->A_csc, h->colptr, h->csc_row, h->n, t, Tin, W, X, V, L->partial, L->order, L->ntiles,
-                                                                         L->tt_ptr, L->tt_src, L->tt_slot);
-    *prow = grid * (gpl::kTileThreads / 32);
-  } else {
-    const int G = lap_groups(t), grid = lap_grid(L->grid_mv, G);
-    gpl::mv_Bt_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->A, h->colptr, h->csc_pos, h->m, h->n, t, G, Tin, W, X, V, L->partial, L->order);
-    *prow = grid * (gpl::kBlock / 32) / G;
-  }
+  const int G = lap_groups(t), grid = lap_grid(L->grid_mv, G);
+  gpl::mv_Bt_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->A, h->colptr, h->csc_pos, h->m, h->n, t, G, Tin, W, X, V, L->partial, L->order);
+  *prow = grid * (gpl::kBlock / 32) / G;
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
   return 0;
@@ -1179,7 +884,6 @@ int lap_mv_Bt(gpbdev_vecchia* h, int t, const double* Tin, const double* W, cons
 int lap_apply_op(gpbdev_vecchia* h, int t, const double* X, double* V, double* Tbuf, double* dots) {
   gpb_laplace_state* L = h->lap;
   const int64_t n = h->n;
-  LapScope scope(t == 1 ? 0 : 2);
   const int G = lap_groups(t), grid = lap_grid(L->grid_mv, G);
   if (t == 1) {
     gpl::v_mv_B_kernel<<<grid, gpl::kBlock, 0, h->stream>>>(h->A, h->nn, h->m, n, h->Dinv, X, Tbuf);
@@ -1202,7 +906,6 @@ int lap_precond(gpbdev_vecchia* h, int t, const double* R, double* Z, double* Yb
   const double* A = h->A; const int32_t* colptr = h->colptr; const int32_t* csc = h->csc_pos; const int32_t* nn = h->nn;
   int m = h->m; int64_t nn_ = n; int tt = t; const double* dw = L->dw; double* partial = L->partial; int* err = L->err;
   const double* Yc = Ybuf;
-  LapScope scope(t == 1 ? 1 : 3);
   if (t == 1) {
     const int fb = (int)std::min<int64_t>((n + 255) / 256, (int64_t)h->num_sms * 16);
     gpl::fill_sentinel_kernel<<<fb, 256, 0, h->stream>>>(Ybuf, n);
@@ -1510,11 +1213,6 @@ int gpbdev_vecchia_laplace_eval(gpbdev_vecchia_t h, int cov_type, double var, do
   }
   out[4] = logdet;
   out[0] = -(mll - 0.5 * logdet);
-  if (g_trace.on) {
-    std::fprintf(stderr, "[laplace n=%lld] op(t=1) %.3fs/%d  precond(t=1) %.3fs/%d  op(t=%d) %.3fs/%d  precond(t=%d) %.3fs/%d\n", (long long)n,
-                 g_trace.t[0], g_trace.c[0], g_trace.t[1], g_trace.c[1], L->t, g_trace.t[2], g_trace.c[2], L->t, g_trace.t[3], g_trace.c[3]);
-    for (int i = 0; i < 8; ++i) { g_trace.t[i] = 0.; g_trace.c[i] = 0; }
-  }
   return 0;
 }
 

@@ -211,7 +211,7 @@ GPBDEV_EXPORT int gpbdev_vecchia_laplace_set_collective(gpbdev_vecchia_t h, void
 /* Read-back of one Laplace operator, for tests (off the hot path). Factors the latent model at (var, range) with its range
  * derivative (A, D^-1, dA, dD; B = I - A, B_grad = -dA), installs W_host (n, Vecchia order) and dw = D^-1 + W, and applies operator
  * `op` to X_host (n x t row-major, Vecchia order, 1 <= t <= 128) through the dispatch the evaluation uses (t = 1 single-vector
- * kernels, tiled kernels where enabled and eligible, the engine's row order):
+ * kernels, otherwise the gather kernels in the engine's row order):
  *   0  out = D^-1 B X                                      3  out = P^-1 X, P = B^T (D^-1 + W) B,  dots = X . out
  *   1  out = B^T X + W X2,            dots = X2 . out      4  out = B^-T X   (the first solve of op 3)
  *   2  out = (B^T D^-1 B + W) X,      dots = X . out       5  out = B_grad X

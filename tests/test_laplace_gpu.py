@@ -47,22 +47,6 @@ def test_negll_matches_reference_golden(idx):
     assert abs(v - c["negll_cholesky"]) <= 2e-3 * abs(c["negll_cholesky"])
 
 
-@pytest.mark.parametrize("variant", ["tiled", "index_order"])
-@pytest.mark.parametrize("idx", [1, 3, 5])
-def test_negll_matches_reference_golden_for_every_operator_variant(idx, variant, monkeypatch):
-    """The multi-vector products with B and B^T exist as gather kernels (rows taken in Morton order by default, by index with
-    GPB200_LAPLACE_ORDER=index) and as tiled kernels that stage the neighbour rows in shared memory with bulk async copies
-    (GPB200_LAPLACE_TILED=1). Same bar as the default path."""
-    env = {"tiled": {"GPB200_LAPLACE_TILED": "1"}, "index_order": {"GPB200_LAPLACE_ORDER": "index"}}[variant]
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    c = GOLD[idx]
-    X, y, off = data_of(c)
-    gm = product_model(c, X)
-    v = gm.neg_log_likelihood(np.array(c["cov_pars"]), y, fixed_effects=off)
-    assert abs(v - c["negll_iterative"]) <= 1e-6 * abs(c["negll_iterative"])
-
-
 @pytest.mark.parametrize("idx", [1, 2])
 def test_mode_and_iterations_match_oracle(idx):
     c = GOLD[idx]

@@ -2,8 +2,8 @@
 
 `gpbdev_vecchia_laplace_apply` factors the latent model, installs W and dw = D^-1 + W and runs one operator through the same
 dispatch the evaluation uses:
-  op 0  D^-1 B X                  lap_mv_B      mv_B_kernel (G = ceil(t/32) column groups), mv_B_tiled_kernel
-  op 1  B^T X + W X2, dots        lap_mv_Bt     mv_Bt_kernel, mv_Bt_tiled_kernel
+  op 0  D^-1 B X                  lap_mv_B      mv_B_kernel (G = ceil(t/32) column groups)
+  op 1  B^T X + W X2, dots        lap_mv_Bt     mv_Bt_kernel
   op 2  (B^T D^-1 B + W) X, dots  lap_apply_op  t = 1: v_mv_B_kernel + v_mv_Bt_kernel, else ops 0 and 1
   op 3  P^-1 X, dots              lap_precond   t = 1: v_trs_bwd_kernel + v_trs_fwd_kernel, else trs_bwd_kernel + trs_fwd_kernel
   op 4  B^-T X                    the first solve of op 3
@@ -33,12 +33,11 @@ Every output must also be free of the solves' sentinel word 0x7ff8dead0badf00d, 
 
 The cases reach every dispatch bucket (test_cases_reach_every_dispatch_bucket restates the dispatch and checks it without a GPU):
 t in {1, 2, 3, 31, 32, 33, 50, 63, 64, 65, 96, 97, 127, 128} (G = 1 ... 4), m in {1, 2, 5, 15, 16, 17, 29, 30}, n from 2 and
-m + 1 (every row padded) up to 1e5, d in {1, 2, 3, 4} (Morton order only at d = 2 and 3), GPB200_LAPLACE_ORDER=index and
-GPB200_LAPLACE_TILED=1 (eligible for even t <= 64), W = 0, W in (0, 0.25] and D^-1 spread over several decades, and hand-built
-neighbour patterns: a chain (depth n - 1, up to n = 1e5), a star (column 0 has n - 1 entries), columns of exactly 15, 16, 17, 31,
-32, 33, 127, 128 and 129 entries (around trs_bwd's 16-entry batches, mv_Bt's 32-entry chunks and v_trs_bwd's 128-entry unrolled
-loop), a comb (depth 1: every row depends on the first 30 rows) and a tiled case whose B and B^T tiles hold more than
-kTileCap = 272 distinct source rows, so that both tiled kernels read sources beyond the tile from global memory.
+m + 1 (every row padded) up to 1e5, d in {1, 2, 3, 4} (Morton order at d = 2 and 3, index order at d = 1 and 4), W = 0,
+W in (0, 0.25] and D^-1 spread over several decades, and hand-built neighbour patterns: a chain (depth n - 1, up to n = 1e5), a
+star (column 0 has n - 1 entries), columns of exactly 15, 16, 17, 31, 32, 33, 127, 128 and 129 entries (around trs_bwd's 16-entry
+batches, mv_Bt's 32-entry chunks and v_trs_bwd's 128-entry unrolled loop) and a comb (depth 1: every row depends on the first 30
+rows).
 
 End to end, GPModel at num_rand_vec_trace = t for t in {1, 2, 31, 32, 33, 64, 65, 97, 128} runs against oracle.laplace with the
 same probe vectors: equal Newton, CG and SLQ iteration counts, log-det within 1e-8, NLL within 1e-9, mode within 1e-5 (the bars of
@@ -59,7 +58,6 @@ LD = np.longdouble
 SENTINEL = 0x7ff8dead0badf00d
 T_ALL = (1, 2, 3, 31, 32, 33, 50, 63, 64, 65, 96, 97, 127, 128)
 OP_NAMES = ("DinvBX", "BtX+WX2", "SigmaI+W", "Pinv", "Bt_inv", "BgX", "X2+BgtX")
-TILE_ROWS, TILE_CAP, SLOT_NONE, SLOT_GLOBAL = 32, 272, 0xFFFF, 0xFFFE
 COL_COUNTS = (15, 16, 17, 31, 32, 33, 127, 128, 129)
 WORST = {}  # op name -> worst error / bar ratio seen in this session
 
@@ -106,20 +104,6 @@ def comb_nn(n, m=30):
     return pad_rows([[] if i < m else list(range(m)) for i in range(n)], m)
 
 
-def overflow_nn(n, m=30):
-    """For coordinates already in Morton order (tile k = rows 32k ... 32k + 31). Tile 40: its 32 rows depend on disjoint sets of
-    30 rows (992 distinct sources of the B tile). Tile 0: its 32 columns have 10 dependents each among rows 2000 ... 2319 (320
-    distinct sources of the B^T tile) besides the dependents from tile 40. Every other row depends on its predecessors."""
-    assert n >= 2320 and m == 30
-    rows = [list(range(max(0, i - 3), i)) for i in range(n)]
-    for r in range(TILE_ROWS):
-        rows[40 * TILE_ROWS + r] = list(range(30 * r, 30 * r + 30))
-    for s in range(320):
-        i = 2000 + s
-        rows[i] = sorted({s % TILE_ROWS} | set(range(i - 3, i)))
-    return pad_rows(rows, m)
-
-
 def depth(nn):
     """length of the longest dependency path"""
     lev = np.zeros(nn.shape[0], dtype=np.int64)
@@ -135,35 +119,16 @@ def col_counts(nn):
 
 
 # ------------------------------------------------------------------------------------------------- dispatch restatement
-def morton_order(coords):
-    """laplace_ensure: Z-curve key over the bounding box (d = 2: 2 x 16 bits, d = 3: 3 x 10 bits), ties by index"""
-    n, d = coords.shape
-    lo, hi = coords.min(0), coords.max(0)
-    bits = 16 if d == 2 else 10
-    span = np.where(hi > lo, hi - lo, 1.)
-    w = np.where(hi > lo, (coords - lo) / span, 0.)
-    q = np.minimum(float((1 << bits) - 1), w * float(1 << bits)).astype(np.uint64)
-    code = np.zeros(n, dtype=np.uint64)
-    for b in range(bits - 1, -1, -1):
-        for k in range(d):
-            code = (code << np.uint64(1)) | ((q[:, k] >> np.uint64(b)) & np.uint64(1))
-    return np.argsort(code, kind="stable")
+def engine_order(d):
+    """laplace_ensure: Morton (Z-curve) order at d = 2 and 3, index order otherwise"""
+    return "morton" if d in (2, 3) else "index"
 
 
-def engine_order(d, env):
-    return "morton" if d in (2, 3) and env.get("GPB200_LAPLACE_ORDER") != "index" else "index"
-
-
-def tiles_on(d, env):
-    return engine_order(d, env) == "morton" and env.get("GPB200_LAPLACE_TILED") == "1"
-
-
-def dispatch(op, t, d, env):
+def dispatch(op, t, d):
     """kernel buckets (family, G, order) one apply runs: lap_mv_B / lap_mv_Bt / lap_apply_op / lap_precond / the gradient launches.
     Only the gather operator kernels take the engine's row order; the single-vector, solve and gradient kernels go by index."""
-    order, G = engine_order(d, env), (t + 31) // 32
-    tiled = tiles_on(d, env) and t > 1 and t % 2 == 0 and t <= 64
-    mv = {("tiled", G, order)} if tiled else {("mv", G, order)}
+    G = (t + 31) // 32
+    mv = {("mv", G, engine_order(d))}
     if op in (0, 1):
         return mv
     if op == 2:
@@ -173,71 +138,42 @@ def dispatch(op, t, d, env):
     return {("grad", G, "index")}
 
 
-ALL_BUCKETS = ({("mv", G, o) for G in (1, 2, 3, 4) for o in ("morton", "index")} | {("tiled", G, "morton") for G in (1, 2)} |
+ALL_BUCKETS = ({("mv", G, o) for G in (1, 2, 3, 4) for o in ("morton", "index")} |
                {("v_mv", 1, "index"), ("v_trs", 1, "index")} | {("trs", G, "index") for G in (1, 2, 3, 4)} |
                {("grad", G, "index") for G in (1, 2, 3, 4)})
 
 
-def tile_slots(order, nn):
-    """lap_build_tiles: per tile of 32 rows of `order` the sorted distinct sources of B (rows and neighbours) and of B^T (the
-    columns' dependents); a source's slot is its rank in that list, SLOT_GLOBAL from kTileCap on. Returns (slotB, slotT)."""
-    n, m = nn.shape
-    rows_e = np.repeat(np.arange(n), m).reshape(n, m)
-    mask = nn >= 0
-    deps = [[] for _ in range(n)]
-    for i, j in zip(rows_e[mask], nn[mask]):
-        deps[j].append(i)
-    slotB, slotT = [], []
-    for p0 in range(0, n, TILE_ROWS):
-        tile = order[p0:p0 + TILE_ROWS]
-        srcB = np.unique(np.concatenate([tile, nn[tile][nn[tile] >= 0]]))
-        srcT = np.unique(np.array([i for j in tile for i in deps[j]], dtype=np.int64))
-        for i in tile:
-            ids = np.concatenate([[i], nn[i][nn[i] >= 0]])
-            k = np.searchsorted(srcB, ids)
-            slotB += list(np.where(k < TILE_CAP, k, SLOT_GLOBAL))
-            if deps[i]:
-                k = np.searchsorted(srcT, deps[i])
-                slotT += list(np.where(k < TILE_CAP, k, SLOT_GLOBAL))
-    return np.array(slotB), np.array(slotT)
-
-
 # ------------------------------------------------------------------------------------------------------------ the cases
-# (name, n, d, m, pattern, env, ts, W regime, covariance id); pattern "knn" = the engine's own neighbour search
-TIL = {"GPB200_LAPLACE_TILED": "1"}
-IDX = {"GPB200_LAPLACE_ORDER": "index"}
+# (name, n, d, m, pattern, ts, W regime, covariance id); pattern "knn" = the engine's own neighbour search
 CASES = [
-    ("tsweep", 600, 2, 15, "knn", {}, T_ALL, "small", 0),
-    ("tsweep-index", 500, 3, 15, "knn", IDX, (1, 3, 33, 65, 97, 128), "small", 1),
-    ("tiled-d2", 800, 2, 15, "knn", TIL, (1, 2, 3, 31, 32, 33, 50, 63, 64, 65, 96), "small", 0),
-    ("tiled-d3", 800, 3, 25, "knn", TIL, (2, 50, 64, 65), "zero", 1),
-    ("n2-m1", 2, 1, 1, "knn", {}, (1, 2, 33), "small", 0),
-    ("n3-m2", 3, 4, 2, "knn", {}, (1, 2, 65), "small", 0),
-    ("n6-m5", 6, 3, 5, "knn", {}, (1, 3, 97), "small", 1),
-    ("n16-m15", 16, 2, 15, "knn", TIL, (1, 2, 64), "small", 0),
-    ("n17-m16", 17, 1, 16, "knn", {}, (1, 32, 128), "small", 0),
-    ("n18-m17", 18, 2, 17, "knn", IDX, (1, 33), "small", 0),
-    ("n30-m29", 30, 3, 29, "knn", {}, (1, 63), "small", 0),
-    ("n31-m30", 31, 4, 30, "knn", {}, (1, 96), "small", 0),
-    ("m30-n5000", 5000, 2, 30, "knn", {}, (1, 50), "small", 0),
-    ("m17-n3000", 3000, 3, 17, "knn", {}, (1, 33), "small", 1),
-    ("m5-n2000", 2000, 1, 5, "knn", {}, (1, 65), "small", 0),
-    ("m16-n2500", 2500, 4, 16, "knn", {}, (1, 32), "small", 0),
-    ("m1-n1500", 1500, 2, 1, "knn", {}, (1, 97), "small", 0),
-    ("m2-n1000", 1000, 3, 2, "knn", TIL, (1, 64, 127), "small", 0),
-    ("m29-n1200", 1200, 1, 29, "knn", {}, (1, 128), "small", 1),
-    ("m15-n900", 900, 4, 15, "knn", {}, (1, 31), "zero", 0),
-    ("w0-d2", 1000, 2, 10, "knn", {}, (1, 64), "zero", 0),
-    ("dinv-spread", 1000, 2, 10, "knn", {}, (1, 33), "small", 3),
-    ("chain-3000", 3000, 2, 1, "chain", {}, (1, 2, 65), "small", 0),
-    ("chain-1e5", 100000, 2, 1, "chain", {}, (1, 50), "small", 0),
-    ("star-5000", 5000, 2, 5, "star", {}, (1, 50), "small", 0),
-    ("colcounts", 600, 2, 2, "cols", {}, (1, 3, 33), "small", 0),
-    ("colcounts-index", 600, 3, 2, "cols", IDX, (1, 64), "zero", 0),
-    ("comb-3000", 3000, 2, 30, "comb", {}, (1, 64), "small", 0),
-    ("tile-overflow", 2400, 2, 30, "overflow", TIL, (1, 2, 33, 64), "small", 0),
+    ("tsweep", 600, 2, 15, "knn", T_ALL, "small", 0),
+    ("tsweep-index", 500, 4, 15, "knn", (1, 3, 33, 65, 97, 128), "small", 1),
+    ("n2-m1", 2, 1, 1, "knn", (1, 2, 33), "small", 0),
+    ("n3-m2", 3, 4, 2, "knn", (1, 2, 65), "small", 0),
+    ("n6-m5", 6, 3, 5, "knn", (1, 3, 97), "small", 1),
+    ("n16-m15", 16, 2, 15, "knn", (1, 2, 64), "small", 0),
+    ("n17-m16", 17, 1, 16, "knn", (1, 32, 128), "small", 0),
+    ("n18-m17", 18, 1, 17, "knn", (1, 33), "small", 0),
+    ("n30-m29", 30, 3, 29, "knn", (1, 63), "small", 0),
+    ("n31-m30", 31, 4, 30, "knn", (1, 96), "small", 0),
+    ("m30-n5000", 5000, 2, 30, "knn", (1, 50), "small", 0),
+    ("m17-n3000", 3000, 3, 17, "knn", (1, 33), "small", 1),
+    ("m5-n2000", 2000, 1, 5, "knn", (1, 65), "small", 0),
+    ("m16-n2500", 2500, 4, 16, "knn", (1, 32), "small", 0),
+    ("m1-n1500", 1500, 2, 1, "knn", (1, 97), "small", 0),
+    ("m2-n1000", 1000, 3, 2, "knn", (1, 64, 127), "small", 0),
+    ("m29-n1200", 1200, 1, 29, "knn", (1, 128), "small", 1),
+    ("m15-n900", 900, 4, 15, "knn", (1, 31), "zero", 0),
+    ("w0-d2", 1000, 2, 10, "knn", (1, 64), "zero", 0),
+    ("dinv-spread", 1000, 2, 10, "knn", (1, 33), "small", 3),
+    ("chain-3000", 3000, 2, 1, "chain", (1, 2, 65), "small", 0),
+    ("chain-1e5", 100000, 2, 1, "chain", (1, 50), "small", 0),
+    ("star-5000", 5000, 2, 5, "star", (1, 50), "small", 0),
+    ("colcounts", 600, 2, 2, "cols", (1, 3, 33), "small", 0),
+    ("colcounts-index", 600, 4, 2, "cols", (1, 64), "zero", 0),
+    ("comb-3000", 3000, 2, 30, "comb", (1, 64), "small", 0),
 ]
-CASE_T = [(c, t) for c in CASES for t in c[6]]
+CASE_T = [(c, t) for c in CASES for t in c[5]]
 
 
 def case_coords(name, n, d, pattern):
@@ -250,14 +186,12 @@ def case_coords(name, n, d, pattern):
         co = np.column_stack([(np.arange(n) + 0.5 * rng.random(n)) / n, 0.05 * rng.random((n, d - 1))])
     else:
         co = rng.random((n, d))
-    if pattern == "overflow":
-        co = co[morton_order(co)]  # Vecchia order = Morton order: tile k is rows 32k ... 32k + 31
     return np.ascontiguousarray(co)
 
 
 def case_nn(n, m, pattern):
     return {"chain": lambda: chain_nn(n), "star": lambda: star_nn(n, m), "cols": lambda: colcount_nn(n),
-            "comb": lambda: comb_nn(n, m), "overflow": lambda: overflow_nn(n, m)}[pattern]()
+            "comb": lambda: comb_nn(n, m)}[pattern]()
 
 
 def case_pars(n, d, pattern, cid):
@@ -419,7 +353,7 @@ def apply(lib, h, cid, var, rt, op, W, X, X2=None):
 
 @functools.lru_cache(maxsize=None)
 def case_inputs(name):
-    (_, n, d, m, pattern, env, ts, wmode, cid), = [c for c in CASES if c[0] == name]
+    (_, n, d, m, pattern, ts, wmode, cid), = [c for c in CASES if c[0] == name]
     co = case_coords(name, n, d, pattern)
     nn = None if pattern == "knn" else case_nn(n, m, pattern)
     rng = np.random.default_rng(n + m)
@@ -433,10 +367,8 @@ def dot_bar(x, v, bar_v):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case,t", CASE_T, ids=["%s-t%d" % (c[0], t) for c, t in CASE_T])
-def test_operator_matches_extended_precision_reference(lib, case, t, monkeypatch):
-    name, n, d, m, pattern, env, _, wmode, cid = case
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_operator_matches_extended_precision_reference(lib, case, t):
+    name, n, d, m, pattern, _, wmode, cid = case
     co, nn, W = case_inputs(name)
     var, rt = case_pars(n, d, pattern, cid)
     h = create(lib, co, m, nn)
@@ -525,8 +457,8 @@ def verify_operators(R, A, Dinv, W, X, X2, run):
 @pytest.mark.parametrize("d,m", [(2, 10), (3, 20), (2, 30), (3, 30)])
 def test_factor_of_rows_padded_beyond_m_matches_oracle(lib, d, m):
     """Supplied neighbour sets may pad any row with -1, also rows i >= m. The factor kernels took every row i >= m of a model with
-    m equal to their capacity (10, 20, 30) for a row without dummy slots and built its covariance block from stale shared memory:
-    the tile-overflow case above returned different D^-1 B X on two identical calls. Regression: rows i >= m keep 1 ... m of their
+    m equal to their capacity (10, 20, 30) for a row without dummy slots and built its covariance block from stale shared memory,
+    so that D^-1 B X differed between two identical calls. Regression: rows i >= m keep 1 ... m of their
     nearest neighbours; the latent factor and its range derivative (one-observation kernel) and the Gaussian likelihood sums (at
     d = 2, m = 30 the two-observation kernel) must match the oracle and repeat bit for bit."""
     n = 700
@@ -672,19 +604,16 @@ def test_probe_count_above_128_is_refused():
 
 # ------------------------------------------------------------------------------------------------------- no GPU needed
 def test_cases_reach_every_dispatch_bucket():
-    reached = {b for (name, n, d, m, pattern, env, ts, _, _) in CASES for t in ts for op in range(7) for b in dispatch(op, t, d, env)}
+    reached = {b for (name, n, d, m, pattern, ts, _, _) in CASES for t in ts for op in range(7) for b in dispatch(op, t, d)}
     assert reached == ALL_BUCKETS, ALL_BUCKETS - reached
-    assert {t for c in CASES for t in c[6]} == set(T_ALL)
+    assert {t for c in CASES for t in c[5]} == set(T_ALL)
     assert {c[3] for c in CASES} >= {1, 2, 5, 15, 16, 17, 29, 30}
     assert {c[2] for c in CASES} == {1, 2, 3, 4}
     assert any(c[1] == 2 for c in CASES) and all(any(c[1] == m + 1 and c[3] == m for c in CASES) for m in (1, 2, 5, 15, 16, 17, 29, 30))
     assert max(c[1] for c in CASES if c[4] == "knn") == 5000
-    assert {c[7] for c in CASES} == {"zero", "small"} and any(c[0] == "dinv-spread" for c in CASES)
-    # the tiled kernels run with fewer and with more than 32 columns, and both even and odd t fall back where they must
-    assert {t for c in CASES if tiles_on(c[2], c[5]) for t in c[6] if t > 1 and t % 2 == 0 and t <= 64} >= {2, 32, 50, 64}
-    assert {t for c in CASES if tiles_on(c[2], c[5]) for t in c[6]} >= {1, 3, 33, 65, 96}
+    assert {c[6] for c in CASES} == {"zero", "small"} and any(c[0] == "dinv-spread" for c in CASES)
     # the long chain runs with the single-vector and the multi-vector solves
-    assert {t for c in CASES if c[4] == "chain" and c[1] == 100000 for t in c[6]} == {1, 50}
+    assert {t for c in CASES if c[4] == "chain" and c[1] == 100000 for t in c[5]} == {1, 50}
 
 
 def test_engineered_patterns_have_the_advertised_shape():
@@ -696,28 +625,11 @@ def test_engineered_patterns_have_the_advertised_shape():
     assert list(cc[:len(COL_COUNTS)]) == list(COL_COUNTS) and set(cc[len(COL_COUNTS):]) <= {0, 1}
     nn = comb_nn(3000)
     assert depth(nn) == 1 and np.all(col_counts(nn)[:30] == 2970) and np.all(col_counts(nn)[30:] == 0)
-    for nn in (chain_nn(50), star_nn(50, 5), colcount_nn(600), comb_nn(100), overflow_nn(2400)):
+    for nn in (chain_nn(50), star_nn(50, 5), colcount_nn(600), comb_nn(100)):
         for i in range(nn.shape[0]):
             r = nn[i][nn[i] >= 0]
             assert np.all(r < i) and len(set(r)) == r.size
         assert np.all(nn >= -1)
-
-
-def test_tile_overflow_case_reads_sources_beyond_the_tile():
-    """lap_build_tiles restated: the overflow case's B tiles and B^T tiles both hold more than kTileCap distinct source rows, so
-    both tiled kernels take some sources from global memory (SLOT_GLOBAL); an ordinary tile of the same engine does not."""
-    (name, n, d, m, pattern, env, ts, _, _), = [c for c in CASES if c[4] == "overflow"]
-    co = case_coords(name, n, d, pattern)
-    order = morton_order(co)
-    assert np.array_equal(order, np.arange(n))  # the coordinates were put in Morton order: tile k = rows 32k ... 32k + 31
-    nn = overflow_nn(n, m)
-    slotB, slotT = tile_slots(order, nn)
-    assert (slotB == SLOT_GLOBAL).sum() > 0 and (slotT == SLOT_GLOBAL).sum() > 0
-    assert (slotB == SLOT_GLOBAL).sum() == 992 - TILE_CAP
-    # the tiles of a pattern with few distinct sources fit
-    sb, st = tile_slots(order[:320], chain_nn(320))
-    assert not (sb == SLOT_GLOBAL).any() and not (st == SLOT_GLOBAL).any()
-    assert tiles_on(d, env) and any(t % 2 == 0 and 2 <= t <= 64 for t in ts)
 
 
 def test_create_rejects_neighbour_sets_that_are_not_earlier_rows(product_lib):

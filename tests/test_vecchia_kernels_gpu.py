@@ -1,16 +1,16 @@
 """Every specialisation of the Vecchia factor kernels against the oracle.
 
 `launch_eval` (gpboost_b200/csrc/dev/dev_api.cu) runs one of several separately compiled kernels, chosen by dimension d,
-neighbour count m, mode and two switches read when the engine is created:
+neighbour count m and mode:
 
   one-observation kernel  vecchia_factor_kernel<COV, MODE, DIM, cap>  DIM = 2 at d = 2 (unrolled gather), DIM = 0 (generic) else;
-                          cap = 10 / 20 / 30 for m <= 10 / <= 20 / <= 30
-  two-observation kernel  vecchia_nll2_kernel<COV, MODE>              d = 2, 20 < m <= 30, modes NLL / STORE / GRAD, unless
-                                                                      GPB200_NLL_KERNEL=1
+                          cap = 10 / 20 / 30 for m <= 10 / <= 20 / <= 30; at d = 2, cap 30 only for MODE_STORE_GRAD
+  two-observation kernel  vecchia_nll2_kernel<COV, MODE>              d = 2, 20 < m <= 30, modes NLL / STORE / GRAD
   big kernel              vecchia_big_kernel<COV, BIG_*>              30 < m <= 60, any d
 
 Each has its own gather, padding and unrolling, for 4 covariances and 4 modes. The cases below reach every (kernel, DIM, cap)
-bucket for every covariance (test_parametrisation_reaches_every_kernel_bucket checks that without a GPU), including the band
+bucket for every covariance and every mode it serves (test_parametrisation_reaches_every_kernel_bucket checks that without a
+GPU), including the band
 edges m = 1, 10/11, 20/21, 30/31/32, rows that are all padding (n = m + 1), distance ties and coincident points.
 
 Tolerances as in tests/test_vecchia_gpu.py: neighbour indices bit-exact; sums, gradients, A, D^-1 and Psi^-1 y <= 1e-8 relative.
@@ -32,37 +32,33 @@ COV_IDS = ["exponential", "matern1.5", "matern2.5", "gaussian"]
 MODE_NLL, MODE_STORE, MODE_GRAD, MODE_STORE_GRAD = 0, 1, 2, 3
 
 
-def kernel_bucket(d, m, mode, nll1_only=False):
-    """(kernel, DIM, cap) that launch_eval runs for one pass; restates dev_api.cu:pick_cap / pick_dim (105-115), the big-kernel
-    branch of launch_eval (m > kMaxNeighbors = 30, :287) and its two-observation branch (:314)."""
+def kernel_bucket(d, m, mode):
+    """(kernel, DIM, cap) that launch_eval runs for one pass; restates dev_api.cu:pick_cap / pick_dim, the big-kernel branch of
+    launch_eval (m > kMaxNeighbors = 30) and its two-observation branch (d = 2, m > 20)."""
     if m > 30:
         return ("big", 0, 60)
-    if mode in (MODE_NLL, MODE_STORE, MODE_GRAD) and d == 2 and m > 20 and not nll1_only:
+    if mode in (MODE_NLL, MODE_STORE, MODE_GRAD) and d == 2 and m > 20:
         return ("two_obs", 2, 30)
     return ("one_obs", 2 if d == 2 else 0, 10 if m <= 10 else (20 if m <= 20 else 30))
 
 
-ALL_BUCKETS = {("one_obs", dim, cap) for dim in (2, 0) for cap in (10, 20, 30)} | {("two_obs", 2, 30), ("big", 0, 60)}
+# (kernel, DIM, cap) run by NLL / STORE / GRAD; ("one_obs", 2, 30) serves MODE_STORE_GRAD only
+ALL_BUCKETS = ({("one_obs", dim, cap) for dim in (2, 0) for cap in (10, 20, 30)} - {("one_obs", 2, 30)}) | {("two_obs", 2, 30), ("big", 0, 60)}
 STORE_GRAD_BUCKETS = {("one_obs", dim, cap) for dim in (2, 0) for cap in (10, 20, 30)}
 
-# (n, d, m, data, env): data "synth" = U[0,1]^d, "dup" = with repeated and coincident points, "lattice3" = 3-D integer grid
-# (distance ties everywhere); env = kernel switches set when the engine is created
-FACTOR_CASES = [(700, d, m, "synth", {}) for d in (1, 2, 3, 5, 16) for m in (1, 10, 11, 20, 21, 30, 31, 32, 60)]
-FACTOR_CASES += [(700, 2, m, "synth", {"GPB200_NLL_KERNEL": "1"}) for m in (21, 25, 30)]
-FACTOR_CASES += [(700, 2, 25, "synth", {}),
-                 (700, 2, 30, "synth", {"GPB200_GRAD_STORES": "0"}), (700, 3, 30, "synth", {"GPB200_GRAD_STORES": "0"}),
-                 (11, 1, 10, "synth", {}), (31, 2, 30, "synth", {}), (31, 2, 30, "synth", {"GPB200_NLL_KERNEL": "1"}),
-                 (26, 3, 25, "synth", {}), (61, 5, 60, "synth", {}),
-                 (900, 3, 25, "dup", {}), (900, 1, 12, "dup", {}), (900, 2, 40, "dup", {}),
-                 (729, 3, 26, "lattice3", {}), (729, 3, 8, "lattice3", {}), (729, 3, 45, "lattice3", {})]
+# (n, d, m, data): data "synth" = U[0,1]^d, "dup" = with repeated and coincident points, "lattice3" = 3-D integer grid
+# (distance ties everywhere)
+FACTOR_CASES = [(700, d, m, "synth") for d in (1, 2, 3, 5, 16) for m in (1, 10, 11, 20, 21, 30, 31, 32, 60)]
+FACTOR_CASES += [(700, 2, 25, "synth"), (11, 1, 10, "synth"), (31, 2, 30, "synth"), (26, 3, 25, "synth"), (61, 5, 60, "synth"),
+                 (900, 3, 25, "dup"), (900, 1, 12, "dup"), (900, 2, 40, "dup"),
+                 (729, 3, 26, "lattice3"), (729, 3, 8, "lattice3"), (729, 3, 45, "lattice3")]
 
 # (d, m): MODE_STORE_GRAD, the latent factor and its range derivative (Laplace path)
 LATENT_CASES = [(d, m) for d in (1, 2, 3, 5) for m in (5, 15, 25, 30)]
 
 
 def case_id(c):
-    n, d, m, data, env = c
-    return "n%d-d%d-m%d-%s%s" % (n, d, m, data, "".join("-%s=%s" % (k[7:], v) for k, v in env.items()))
+    return "n%d-d%d-m%d-%s" % c
 
 
 def P(a, t=C.c_double):
@@ -134,8 +130,8 @@ def check_engine_against_oracle(lib, h, perm, co, y, m, cov, shape, cp):
         assert np.abs(ya - ya_o).max() <= REL * np.abs(ya_o).max()
 
     out = np.zeros(9)
-    # STORE first (factor of the STORE pass), then GRAD: the two-observation gradient pass stores A, D^-1 and u again
-    # (unless GPB200_GRAD_STORES=0), and the factor is read once more after it
+    # STORE first (factor of the STORE pass), then GRAD: the two-observation gradient pass stores A, D^-1 and u again, and the
+    # factor is read once more after it
     for mode in (MODE_STORE, MODE_GRAD, MODE_NLL):
         chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(pt[1]), mode, P(out)))
         assert abs(out[0] - ref[1]) <= REL * abs(ref[1]), mode
@@ -152,10 +148,8 @@ def check_engine_against_oracle(lib, h, perm, co, y, m, cov, shape, cp):
 @pytest.mark.gpu
 @pytest.mark.parametrize("cov,shape", COVS, ids=COV_IDS)
 @pytest.mark.parametrize("case", FACTOR_CASES, ids=[case_id(c) for c in FACTOR_CASES])
-def test_factor_kernel_matches_oracle(lib, cov, shape, case, monkeypatch):
-    n, d, m, data, env = case
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_factor_kernel_matches_oracle(lib, cov, shape, case):
+    n, d, m, data = case
     coords, y = case_coords(n, d, data, 13 + d)
     h, perm, co = make_engine(lib, coords, m)
     try:
@@ -165,39 +159,26 @@ def test_factor_kernel_matches_oracle(lib, cov, shape, case, monkeypatch):
 
 
 @pytest.mark.gpu
-def test_kernel_switches_are_per_engine(lib, monkeypatch):
-    """GPB200_NLL_KERNEL and GPB200_GRAD_STORES are read when an engine is created: engines with either setting live side by side
-    in one process and each matches the oracle. Which kernel ran is visible from the outside: only the two-observation gradient
-    pass with stores on writes the factor (into buffers a STORE pass allocated), so a STORE request at the parameters of that
-    gradient pass launches nothing on that engine alone."""
+def test_store_after_gradient_pass_launches_nothing(lib):
+    """The two-observation gradient pass (d = 2, 20 < m <= 30) also writes the factor into the buffers a STORE pass allocated, so
+    a STORE request at the parameters of that gradient pass launches nothing; the engine then still matches the oracle."""
     coords, y = datagen.synth(800, 2, 7)
     m, cov, shape = 30, "matern", 1.5
     cp = [0.4, 1.3, spread_range(800, 2)]
     cid = ov.cov_id(cov, shape)
     _, pt = ov.transform_cov_pars(cp, cov, shape)
-    engines = {}
-    for name, env in (("default", {}), ("nll1", {"GPB200_NLL_KERNEL": "1"}), ("no_stores", {"GPB200_GRAD_STORES": "0"})):
-        monkeypatch.delenv("GPB200_NLL_KERNEL", raising=False)
-        monkeypatch.delenv("GPB200_GRAD_STORES", raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
-        engines[name] = make_engine(lib, coords, m)
-    monkeypatch.delenv("GPB200_NLL_KERNEL", raising=False)
-    monkeypatch.delenv("GPB200_GRAD_STORES", raising=False)
+    h, perm, co = make_engine(lib, coords, m)
     try:
         out = np.zeros(9)
-        for name, (h, perm, co) in engines.items():
-            chk(lib, lib.gpbdev_vecchia_set_y(h, P(np.ascontiguousarray(y))))
-            chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(1.5 * pt[1]), MODE_STORE, P(out)))
-            chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(pt[1]), MODE_GRAD, P(out)))
-            before = lib.gpbdev_vecchia_launch_count(h)
-            chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(pt[1]), MODE_STORE, P(out)))
-            assert (lib.gpbdev_vecchia_launch_count(h) == before) == (name == "default"), name
-        for name, (h, perm, co) in engines.items():
-            check_engine_against_oracle(lib, h, perm, co, y, m, cov, shape, cp)
+        chk(lib, lib.gpbdev_vecchia_set_y(h, P(np.ascontiguousarray(y))))
+        chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(1.5 * pt[1]), MODE_STORE, P(out)))
+        chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(pt[1]), MODE_GRAD, P(out)))
+        before = lib.gpbdev_vecchia_launch_count(h)
+        chk(lib, lib.gpbdev_vecchia_eval(h, cid, C.c_double(pt[0]), C.c_double(pt[1]), MODE_STORE, P(out)))
+        assert lib.gpbdev_vecchia_launch_count(h) == before
+        check_engine_against_oracle(lib, h, perm, co, y, m, cov, shape, cp)
     finally:
-        for h, _, _ in engines.values():
-            lib.gpbdev_vecchia_free(h)
+        lib.gpbdev_vecchia_free(h)
 
 
 def latent_coords(n, d, seed):
@@ -252,23 +233,19 @@ def test_latent_factor_derivative_rejects_more_than_30_neighbours(lib, m):
 
 
 # ---------------------------------------------------------------------------------------- Laplace off the plane
-# (d, covariance, shape, n, m, operator switches): d = 3 takes the Morton-ordered operator kernels by default
-LAPLACE_CASES = [(1, "exponential", 0.5, 2000, 20, {}),
-                 (3, "matern", 1.5, 2500, 25, {}),
-                 (3, "matern", 1.5, 2500, 25, {"GPB200_LAPLACE_ORDER": "index"}),
-                 (3, "matern", 1.5, 2500, 25, {"GPB200_LAPLACE_TILED": "1"}),
-                 (4, "gaussian", 0., 1500, 15, {})]
+# (d, covariance, shape, n, m): d = 3 takes the Morton-ordered operator kernels, d = 1 and 4 the index-ordered ones
+LAPLACE_CASES = [(1, "exponential", 0.5, 2000, 20),
+                 (3, "matern", 1.5, 2500, 25),
+                 (4, "gaussian", 0., 1500, 15)]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", LAPLACE_CASES, ids=lambda c: "d%d-%s%s" % (c[0], c[1], "".join("-" + v for v in c[5].values())))
-def test_laplace_off_the_plane_matches_oracle(case, monkeypatch):
+@pytest.mark.parametrize("case", LAPLACE_CASES, ids=lambda c: "d%d-%s" % (c[0], c[1]))
+def test_laplace_off_the_plane_matches_oracle(case):
     """bernoulli_logit at d = 1, 3, 4 against oracle.laplace.negll (iterative), on the bar of
     tests/test_laplace_gpu.py::test_mode_and_iterations_match_oracle"""
     from gpboost_b200 import GPModel
-    d, cov, shape, n, m, env = case
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+    d, cov, shape, n, m = case
     X, y, _ = datagen.binary_synth(n, 30 + d, False, d=d)
     cp = [1.0, spread_range(n, d)]
     gm = GPModel(likelihood="bernoulli_logit", gp_coords=X, cov_function=cov, cov_fct_shape=shape, gp_approx="vecchia",
@@ -315,17 +292,15 @@ def test_prediction_off_the_plane_matches_oracle(cov, shape, d):
 def test_parametrisation_reaches_every_kernel_bucket():
     """Every (kernel, DIM, cap) bucket of launch_eval is run for every covariance and every mode it serves, so trimming the
     cases above cannot silently drop one."""
-    reached = {(b, mode) for n, d, m, _, env in FACTOR_CASES for mode in (MODE_NLL, MODE_STORE, MODE_GRAD)
-               for b in [kernel_bucket(d, m, mode, env.get("GPB200_NLL_KERNEL") == "1")]}
+    reached = {(kernel_bucket(d, m, mode), mode) for n, d, m, _ in FACTOR_CASES for mode in (MODE_NLL, MODE_STORE, MODE_GRAD)}
     assert reached == {(b, mode) for b in ALL_BUCKETS for mode in (MODE_NLL, MODE_STORE, MODE_GRAD)}
     latent = {kernel_bucket(d, m, MODE_STORE_GRAD) for d, m in LATENT_CASES}
     assert latent == STORE_GRAD_BUCKETS
-    # the one-observation cap-30 kernel at d = 2 serves NLL / STORE / GRAD only with the switch; the GRAD_STORES=0 path is run at
-    # d = 2 (two-observation kernel) and at d = 3
-    assert any(d == 2 and 20 < m <= 30 and env.get("GPB200_NLL_KERNEL") == "1" for _, d, m, _, env in FACTOR_CASES)
-    assert {d for _, d, _, _, env in FACTOR_CASES if env.get("GPB200_GRAD_STORES") == "0"} >= {2, 3}
+    # the one-observation cap-30 kernel at d = 2 serves MODE_STORE_GRAD only: NLL / STORE / GRAD there take the two-observation kernel
+    assert ("one_obs", 2, 30) in STORE_GRAD_BUCKETS
+    assert all(b != ("one_obs", 2, 30) for b, _ in reached)
     # band edges and padded rows
-    ms = {m for _, _, m, _, _ in FACTOR_CASES}
+    ms = {m for _, _, m, _ in FACTOR_CASES}
     assert {1, 10, 11, 20, 21, 30, 31, 32, 60} <= ms
-    assert any(n <= m + 1 for n, _, m, _, _ in FACTOR_CASES)
-    assert {d for _, d, _, _, _ in FACTOR_CASES} >= {1, 2, 3, 5, 16}
+    assert any(n <= m + 1 for n, _, m, _ in FACTOR_CASES)
+    assert {d for _, d, _, _ in FACTOR_CASES} >= {1, 2, 3, 5, 16}
