@@ -226,3 +226,5 @@ int gpbdev_grouped_yaux_device(gpbdev_grouped_t h, double var_ratio, double scal
 int64_t gpbdev_grouped_launch_count(gpbdev_grouped_t h) { return h ? h->launches : 0; }
 
 }  // extern "C"
+
+#include "grouped_multi.cuh"

@@ -102,7 +102,7 @@ class REModel {
   const std::string& OptimizerCovPars() const { return optimizer_; }
   int64_t NumLikelihoodEvals() const { return num_ll_evals_; }
   gpbdev_vecchia_t Engine() const { return engine_; }
-  bool IsGrouped() const { return grouped_ != nullptr; }
+  bool IsGrouped() const { return grouped_ != nullptr || gmulti_ != nullptr; }
   // transformed <-> original scale (cov_fcts.h:485-623)
   void TransformCovPars(const double* orig, double* trans) const;
   void TransformBackCovPars(const double* trans, double* orig) const;
@@ -173,6 +173,20 @@ class REModel {
   double gsums_[5];
   void CreateGroupedBackend(const char* re_group_data);
   void GroupedPass(double var_ratio);
+  // K >= 2 grouped random effects (crossed or nested): iterative method with the SSOR preconditioner on the device
+  gpbdev_grouped_multi_t gmulti_ = nullptr;
+  int num_re_group_ = 0;
+  int gm_num_levels_total_ = 0;
+  bool gm_probes_saved_ = false;
+  int gm_probes_t_ = 0;
+  // the reference warm-starts M x = Z^T y from the previous solution while its optimiser iteration counter num_iter_ is positive
+  // (re_model_template.h:9852): set by the L-BFGS driver from its second iteration on, cleared when a fit starts
+  bool gm_warm_ = false;
+  void CreateGroupedMultiBackend(const char* re_group_data);
+  void GmEnsureProbes();
+  // one device evaluation at the transformed variance ratios v (K values): sums_ QUAD / LOGDET, laplace_out_ CG counts
+  void GroupedMultiPass(const double* v);
+  void GmCfg(double* cfg4) const;
 
   // state (all covariance parameters kept on the TRANSFORMED scale like REModel::cov_pars_)
   std::vector<double> cov_pars_, init_cov_pars_;

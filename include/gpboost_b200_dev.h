@@ -271,6 +271,36 @@ GPBDEV_EXPORT int gpbdev_grouped_yaux_device(gpbdev_grouped_t h, double var_rati
 GPBDEV_EXPORT int64_t gpbdev_grouped_launch_count(gpbdev_grouped_t h);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * K >= 2 grouped random effects (crossed or nested), Gaussian likelihood, iterative method with the SSOR preconditioner:
+ * M = Sigma^-1 + Z^T Z of size G = sum_k G_k in component order (re_model_template.h:9422-9438, :9850-9891, :3033-3124,
+ * :2530-2619). Errors: gpbdev_grouped_last_error. level_index: host, K x n int32 (factor k at k*n), entries in [0, num_levels[k]).
+ */
+typedef struct gpbdev_grouped_multi* gpbdev_grouped_multi_t;
+GPBDEV_EXPORT int gpbdev_grouped_multi_create(gpbdev_grouped_multi_t* out, int device, int64_t n, int K, const int32_t* level_index,
+                                              const int* num_levels);
+GPBDEV_EXPORT int gpbdev_grouped_multi_free(gpbdev_grouped_multi_t h);
+/* out2 = { G, non-zeros of the off-diagonal part of Z^T Z } */
+GPBDEV_EXPORT int gpbdev_grouped_multi_info(gpbdev_grouped_multi_t h, int64_t* out2);
+/* response in original order (host / device pointer): Z_k^T y of every factor and y^T y */
+GPBDEV_EXPORT int gpbdev_grouped_multi_set_y(gpbdev_grouped_multi_t h, const double* y_host);
+GPBDEV_EXPORT int gpbdev_grouped_multi_set_y_device(gpbdev_grouped_multi_t h, const double* y_dev);
+/* probe vectors r ~ N(0, I): G x t column-major (the reference's rand_vec_probe_), 1 <= t <= 128 */
+GPBDEV_EXPORT int gpbdev_grouped_multi_set_probes(gpbdev_grouped_multi_t h, const double* probes, int t);
+/* at variance ratios v[K] = sigma_k^2 / sigma^2; cfg = { cg_max_num_it, cg_max_num_it_tridiag, cg_delta_conv, warm start (0/1) };
+ * out5 = { y'Psi^-1 y, log|Psi|, CG iterations of M x = Z^T y, CG iterations of the Lanczos block, SLQ estimate of log|P^-1 M| } */
+GPBDEV_EXPORT int gpbdev_grouped_multi_eval(gpbdev_grouped_multi_t h, const double* v, const double* cfg, double* out5);
+/* after eval: gradient w.r.t. log v_k (K values) at error variance sigma2 */
+GPBDEV_EXPORT int gpbdev_grouped_multi_grad(gpbdev_grouped_multi_t h, double sigma2, double* grad);
+/* Psi^-1 y * scale in original order into out (device pointer when out_is_device); one more CG solve; *its (may be null) = its count */
+GPBDEV_EXPORT int gpbdev_grouped_multi_yaux(gpbdev_grouped_multi_t h, const double* v, const double* cfg, double scale, double* out,
+                                            int out_is_device, int* its);
+/* test hook: Y = op(X) on host G x t row-major blocks: 0 M X, 1 P^-1 X, 2 L D^-1/2 X, 3 D^-1 upper(M) X; 4: Y = the last x = M^-1 Z^T y */
+GPBDEV_EXPORT int gpbdev_grouped_multi_apply(gpbdev_grouped_multi_t h, const double* v, int which, const double* X, int t, double* Y);
+/* bench hook: mean device time of one M X and one P^-1 X on the probe block, after an eval */
+GPBDEV_EXPORT int gpbdev_grouped_multi_time_ops(gpbdev_grouped_multi_t h, int reps, float* out_ms);
+GPBDEV_EXPORT int64_t gpbdev_grouped_multi_launch_count(gpbdev_grouped_multi_t h);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Device tree learner (dense uint8 bins, numerical features, no missing values, constant hessian).
  * Seam: the reference's TreeLearner interface (include/LightGBM/tree_learner.h:29-117: Init / Train / AddPredictionToScore /
  * GetDataLeafIndices), selected there by device_type (src/LightGBM/treelearner/tree_learner.cpp:15-52).
