@@ -80,9 +80,16 @@ class GPModel(object):
         self.num_neighbors = -1 if num_neighbors is None else int(num_neighbors)
         self.num_parallel_threads = -1 if num_parallel_threads is None else int(num_parallel_threads)
         gauss = likelihood in ("gaussian", "regression")
-        self.num_cov_pars = (1 if gauss else 0) + self.num_group_re + 2 * self.num_gp
+        # GP parameter names as in the reference package (basic.py:5040-5070): one range per coordinate for the ARD kernels, a time and
+        # a space range for the space-time kernel
+        gp_names = ["GP_var", "GP_range"]
+        if cov_function in ("matern_space_time", "exponential_space_time", "Matern_space_time"):
+            gp_names = ["GP_var", "GP_range_time", "GP_range_space"]
+        elif cov_function in ("matern_ard", "gaussian_ard", "exponential_ard", "Matern_ard"):
+            gp_names = ["GP_var"] + ["GP_range_" + str(i + 1) for i in range(self.dim_coords)]
+        self.num_cov_pars = (1 if gauss else 0) + self.num_group_re + (len(gp_names) if self.num_gp else 0)
         self.cov_par_names = (["Error_term"] if gauss else []) + ["Group_%d" % (k + 1) for k in range(self.num_group_re)] + \
-            (["GP_var", "GP_range"] if self.num_gp else [])
+            (gp_names if self.num_gp else [])
         self.params = dict(_DEFAULT_PARAMS)
         self.num_coef = 0
         self.num_covariates = 0
@@ -263,6 +270,12 @@ class GPModel(object):
         it = ctypes.c_int(0)
         self._safe_call(self._LIB.GPB_GetNumIt(self.handle, ctypes.byref(it)))
         return it.value
+
+    def _get_num_neighbor_searches(self):
+        """searches of the Vecchia neighbour sets in the scaled space of an anisotropic kernel (GPB200_GetNumNeighborSearches)"""
+        c = ctypes.c_int(0)
+        self._safe_call(self._LIB.GPB200_GetNumNeighborSearches(self.handle, ctypes.byref(c)))
+        return c.value
 
     def _get_likelihood_name(self):
         buf = ctypes.create_string_buffer(256)

@@ -44,12 +44,13 @@ __global__ void gather_perm_kernel(const double* __restrict__ src, const int32_t
     dst[i] = src[perm[i]];
 }
 
-// fixed-order reduction of the per-warp partial sums: deterministic for a given grid
+// fixed-order reduction of the per-warp partial sums (NACC per row): deterministic for a given grid
+template <int NACC = gpb::kNumAcc>
 __global__ void reduce_partials_kernel(const double* __restrict__ partials, int64_t nrows, double* __restrict__ out) {
   __shared__ double sh[256];
-  for (int k = 0; k < gpb::kNumAcc; ++k) {
+  for (int k = 0; k < NACC; ++k) {
     double s = 0.;
-    for (int64_t r = threadIdx.x; r < nrows; r += blockDim.x) s += partials[r * gpb::kNumAcc + k];
+    for (int64_t r = threadIdx.x; r < nrows; r += blockDim.x) s += partials[r * NACC + k];
     sh[threadIdx.x] = s;
     __syncthreads();
     for (int o = blockDim.x / 2; o > 0; o >>= 1) {
@@ -107,8 +108,8 @@ FactorKernel pick_cap(int m) {
   if (m <= 10) return gpb::vecchia_factor_kernel<COV, MODE, DIM, 10>;
   if (m <= 20) return gpb::vecchia_factor_kernel<COV, MODE, DIM, 20>;
   // d = 2, 20 < m <= 30: NLL / STORE / GRAD run the two-observation kernel (vecchia_nll2.cuh), so only the factor-derivative
-  // modes are instantiated at this cap
-  if constexpr (DIM == 2 && MODE != gpb::MODE_STORE_GRAD && MODE != gpb::MODE_STORE_GRAD2) return nullptr;
+  // modes and the anisotropic gradient are instantiated at this cap
+  if constexpr (DIM == 2 && MODE != gpb::MODE_STORE_GRAD && MODE != gpb::MODE_STORE_GRAD2 && MODE != gpb::MODE_GRAD_ANISO) return nullptr;
   else return gpb::vecchia_factor_kernel<COV, MODE, DIM, 30>;
 }
 template <int COV, int MODE>
@@ -122,6 +123,7 @@ FactorKernel pick_mode(int mode, int d, int m) {
     case gpb::MODE_STORE: return pick_dim<COV, gpb::MODE_STORE>(d, m);
     case gpb::MODE_GRAD: return pick_dim<COV, gpb::MODE_GRAD>(d, m);
     case gpb::MODE_STORE_GRAD2: return pick_dim<COV, gpb::MODE_STORE_GRAD2>(d, m);
+    case gpb::MODE_GRAD_ANISO: return pick_dim<COV, gpb::MODE_GRAD_ANISO>(d, m);
     default: return pick_dim<COV, gpb::MODE_STORE_GRAD>(d, m);
   }
 }
@@ -141,6 +143,7 @@ BigKernel pick_big_mode(int mode) {
     case gpb::BIG_NLL: return gpb::vecchia_big_kernel<COV, gpb::BIG_NLL>;
     case gpb::BIG_STORE: return gpb::vecchia_big_kernel<COV, gpb::BIG_STORE>;
     case gpb::BIG_GRAD: return gpb::vecchia_big_kernel<COV, gpb::BIG_GRAD>;
+    case gpb::BIG_GRAD_ANISO: return gpb::vecchia_big_kernel<COV, gpb::BIG_GRAD_ANISO>;
     default: return gpb::vecchia_big_kernel<COV, gpb::BIG_PRED>;
   }
 }
@@ -168,7 +171,10 @@ struct gpbdev_vecchia {
   int num_sms = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  double* coords = nullptr;   // n x d
+  double* coords = nullptr;   // n x d; for anisotropic kernels the coordinates scaled by gpbdev_vecchia_set_coord_scale
+  double* coords_orig = nullptr;  // n x d unscaled copy (lazy, first gpbdev_vecchia_set_coord_scale)
+  double* partials_aniso = nullptr;  // grid_cap * kWarpsPerBlock x kAnisoAcc (lazy, gpbdev_vecchia_eval_grad_aniso)
+  bool nn_searched = true;    // false from gpbdev_vecchia_create_unsearched until the first gpbdev_vecchia_search_neighbors
   int32_t* nn = nullptr;      // n x m
   int32_t* perm = nullptr;    // n
   double* y_in = nullptr;     // n staging (original order)
@@ -258,6 +264,7 @@ int ensure_csc(gpbdev_vecchia* h) {
 int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int mode, bool latent = false) {
   if (cov_type < 0 || cov_type > 3) return fail("gpbdev_vecchia_eval: unknown covariance id");
   if (mode < 0 || mode > 3) return fail("gpbdev_vecchia_eval: unknown mode");
+  if (!h->nn_searched) return fail("gpbdev_vecchia_eval: the neighbour sets have not been searched (gpbdev_vecchia_search_neighbors)");
   if (!(var > 0.) || !(range > 0.)) return fail("gpbdev_vecchia_eval: covariance parameters must be positive");
   CUDA_TRY(cudaSetDevice(h->device));
   // GPBoost iteration: OptimCovPar's last accepted trial was a gradient pass at the final parameters on this response, and
@@ -381,8 +388,12 @@ int gpbdev_device_count(void) {
   return c;
 }
 
-int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
-                          const int32_t* perm, const int32_t* nn, int64_t row_begin, int64_t row_end) {
+}  // extern "C"
+
+namespace {
+
+int vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered, const int32_t* perm,
+                   const int32_t* nn, int64_t row_begin, int64_t row_end, bool search) {
   if (!out || !coords_ordered || !perm) return fail("gpbdev_vecchia_create: null argument");
   if (n <= 0 || d <= 0 || d > 16) return fail("gpbdev_vecchia_create: need n > 0 and 1 <= dim <= 16");
   if (m < 1 || m > gpb::kBigMaxNeighbors)
@@ -437,6 +448,9 @@ int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, i
   if (nn) {
     CUDA_TRY(cudaMemcpy(h->nn, nn, sizeof(int32_t) * n * m, cudaMemcpyHostToDevice));
     h->nn_host.assign(nn, nn + (size_t)n * m);
+  } else if (!search) {
+    CUDA_TRY(cudaMemset(h->nn, 0xff, sizeof(int32_t) * n * m));
+    h->nn_searched = false;
   } else {
     std::string err;
     gpb::KnnInfo info;
@@ -450,6 +464,20 @@ int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, i
   return 0;
 }
 
+}  // namespace
+
+extern "C" {
+
+int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
+                          const int32_t* perm, const int32_t* nn, int64_t row_begin, int64_t row_end) {
+  return vecchia_create(out, device, n, d, m, coords_ordered, perm, nn, row_begin, row_end, true);
+}
+
+int gpbdev_vecchia_create_unsearched(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
+                                     const int32_t* perm, int64_t row_begin, int64_t row_end) {
+  return vecchia_create(out, device, n, d, m, coords_ordered, perm, nullptr, row_begin, row_end, false);
+}
+
 int gpbdev_vecchia_free(gpbdev_vecchia_t h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
@@ -460,6 +488,7 @@ int gpbdev_vecchia_free(gpbdev_vecchia_t h) {
   cudaFree(h->csc_row); cudaFree(h->A_csc);
   cudaFree(h->X); cudaFree(h->y0); cudaFree(h->gram_partial); cudaFree(h->gram_out); cudaFree(h->quad_partial);
   cudaFree(h->partials); cudaFree(h->sums); cudaFree(h->flush);
+  cudaFree(h->coords_orig); cudaFree(h->partials_aniso);
   cudaFreeHost(h->sums_host); cudaFreeHost(h->stage_host);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -733,6 +762,139 @@ int gpbdev_vecchia_sync(gpbdev_vecchia_t h) {
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   return 0;
 }
+// ---- anisotropic kernels (ARD / space-time): scaled coordinates, neighbour sets searched in the scaled space, per-group gradient
+
+}  // extern "C"
+
+namespace {
+
+struct CoordScale {
+  double s[16];
+};
+
+// dst = src * s[column], one rounded multiply per entry: the same single operation as the host's scaling, so both agree bitwise
+__global__ void scale_coords_kernel(const double* __restrict__ src, double* __restrict__ dst, int64_t n, int d, CoordScale s) {
+  const int64_t nd = n * d;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nd; e += (int64_t)gridDim.x * blockDim.x)
+    dst[e] = __dmul_rn(src[e], s.s[e % d]);
+}
+
+// every view derived from the parameters or the neighbour sets is stale: the STORE shortcut, the stored factor, the CSC pattern
+void drop_factor_state(gpbdev_vecchia* h) {
+  h->factor_stored = false;
+  h->stored_cov = -1; h->last_cov = -1;
+}
+
+}  // namespace
+
+extern "C" {
+
+int gpbdev_vecchia_set_coord_scale(gpbdev_vecchia_t h, const double* scale) {
+  if (!h || !scale) return fail("gpbdev_vecchia_set_coord_scale: null argument");
+  CoordScale cs;
+  for (int k = 0; k < 16; ++k) cs.s[k] = k < h->d ? scale[k] : 0.;
+  for (int k = 0; k < h->d; ++k)
+    if (!(cs.s[k] > 0.) || !std::isfinite(cs.s[k])) return fail("gpbdev_vecchia_set_coord_scale: scale factors must be positive and finite");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (!h->coords_orig) {
+    CUDA_TRY(cudaMalloc(&h->coords_orig, sizeof(double) * h->n * h->d));
+    CUDA_TRY(cudaMemcpyAsync(h->coords_orig, h->coords, sizeof(double) * h->n * h->d, cudaMemcpyDeviceToDevice, h->stream));
+  }
+  scale_coords_kernel<<<h->num_sms * 8, 256, 0, h->stream>>>(h->coords_orig, h->coords, h->n, h->d, cs);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  drop_factor_state(h);
+  return 0;
+}
+
+int gpbdev_vecchia_search_neighbors(gpbdev_vecchia_t h) {
+  if (!h) return fail("gpbdev_vecchia_search_neighbors: null handle");
+  if (h->row_begin != 0 || h->row_end != h->n) return fail("gpbdev_vecchia_search_neighbors: needs the whole model on this device");
+  CUDA_TRY(cudaSetDevice(h->device));
+  std::vector<double> ch((size_t)h->n * h->d);  // the search replays ties on the host copy of the same coordinates
+  CUDA_TRY(cudaMemcpyAsync(ch.data(), h->coords, sizeof(double) * h->n * h->d, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  std::string err;
+  gpb::KnnInfo info;
+  const int nl = gpb::knn_vecchia_search(h->coords, ch.data(), h->n, h->d, h->m, h->nn, h->stream, h->num_sms, &info, &err,
+                                         /*q_begin=*/0, /*end_search_at=*/h->n - 2);
+  if (nl < 0) return fail("gpbdev_vecchia_search_neighbors: device neighbour search failed: " + err);
+  h->launches += nl;
+  h->knn_replayed = (int)info.replayed;
+  h->nn_searched = true;
+  // views of the old sets: host copy, CSC pattern (and the buffers built with it), Laplace state
+  h->nn_host.clear();
+  cudaFree(h->colptr); cudaFree(h->csc_pos); cudaFree(h->yaux); cudaFree(h->csc_row); cudaFree(h->A_csc);
+  h->colptr = nullptr; h->csc_pos = nullptr; h->yaux = nullptr; h->csc_row = nullptr; h->A_csc = nullptr;
+  laplace_release(h);
+  drop_factor_state(h);
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+int gpbdev_vecchia_eval_grad_aniso(gpbdev_vecchia_t h, int cov_type, double var, const int32_t* group_of_coord, int ngroups,
+                                   double* out) {
+  if (!h || !group_of_coord || !out) return fail("gpbdev_vecchia_eval_grad_aniso: null argument");
+  if (cov_type < 0 || cov_type > 3) return fail("gpbdev_vecchia_eval_grad_aniso: unknown covariance id");
+  if (!(var > 0.)) return fail("gpbdev_vecchia_eval_grad_aniso: covariance parameters must be positive");
+  if (ngroups < 1 || ngroups > gpb::kMaxAnisoGroups) return fail("gpbdev_vecchia_eval_grad_aniso: need 1 <= number of groups <= 16");
+  if (!h->nn_searched) return fail("gpbdev_vecchia_eval_grad_aniso: the neighbour sets have not been searched (gpbdev_vecchia_search_neighbors)");
+  unsigned mask[gpb::kMaxAnisoGroups] = {0u};
+  for (int k = 0; k < h->d; ++k) {
+    if (group_of_coord[k] < 0 || group_of_coord[k] >= ngroups) return fail("gpbdev_vecchia_eval_grad_aniso: coordinate group out of range");
+    mask[group_of_coord[k]] |= 1u << k;
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  const int64_t rows_cap = (int64_t)h->grid_cap * gpb::kWarpsPerBlock;
+  if (!h->partials_aniso)  // partial rows, then the reduced sums
+    CUDA_TRY(cudaMalloc(&h->partials_aniso, sizeof(double) * (rows_cap + 1) * gpb::kAnisoAcc));
+  double* sums = h->partials_aniso + rows_cap * gpb::kAnisoAcc;
+  CUDA_TRY(cudaMemcpyToSymbolAsync(gpb::g_aniso_ngroups, &ngroups, sizeof(int), 0, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaMemcpyToSymbolAsync(gpb::g_aniso_mask, mask, sizeof(mask), 0, cudaMemcpyHostToDevice, h->stream));
+  const double range = 1.;  // the isotropic closed form at unit range on the scaled coordinates
+  int64_t rows = 0;
+  if (h->m > gpb::kMaxNeighbors) {
+    gpb::BigArgs b;
+    b.coords = h->coords; b.y = h->y; b.nn = h->nn; b.qcoords = nullptr;
+    b.A = nullptr; b.Dinv = nullptr; b.w = nullptr; b.pred_mean = nullptr; b.pred_var = nullptr; b.partials = h->partials_aniso;
+    b.row_begin = h->row_begin; b.row_end = h->row_end; b.m = h->m; b.d = h->d;
+    b.var = var; b.range = range; b.diag_nb = var + 1.; b.diag_obs = var + 1.;
+    const int warps = 2;
+    BigKernel bk = pick_big_kernel(cov_type, gpb::BIG_GRAD_ANISO);
+    const size_t bsmem = gpb::big_smem_bytes(gpb::BIG_GRAD_ANISO, warps, h->d);
+    CUDA_TRY(cudaFuncSetAttribute(bk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bsmem));
+    int grid = std::max(1, std::min(h->num_sms, (int)(rows_cap / warps)));
+    bk<<<grid, warps * 32, bsmem, h->stream>>>(b);
+    rows = (int64_t)grid * warps;
+  } else {
+    gpb::FactorArgs a;
+    a.coords = h->coords; a.nn = h->nn; a.y = h->y;
+    a.A = nullptr; a.Dinv = nullptr; a.w = nullptr;
+    a.partials = h->partials_aniso;
+    a.n = h->n; a.row_begin = h->row_begin; a.row_end = h->row_end;
+    a.m = h->m; a.d = h->d; a.var = var; a.range = range;
+    a.diag_nb = var + 1.; a.diag_obs = var + 1.;
+    FactorKernel k = pick_kernel(cov_type, gpb::MODE_GRAD_ANISO, h->d, h->m);
+    if (!k) return fail("gpbdev_vecchia_eval_grad_aniso: no factor kernel for this shape");
+    const size_t smem = sizeof(double) * gpb::kWarpsPerBlock * (32 * gpb::kLd + 32 * h->d + 64);
+    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, gpb::kWarpsPerBlock * 32, smem));
+    int grid = std::min(std::max(per_sm, 1) * h->num_sms, h->grid_cap);
+    k<<<grid, gpb::kWarpsPerBlock * 32, smem, h->stream>>>(a);
+    rows = (int64_t)grid * gpb::kWarpsPerBlock;
+  }
+  CUDA_TRY(cudaGetLastError());
+  reduce_partials_kernel<gpb::kAnisoAcc><<<1, 256, 0, h->stream>>>(h->partials_aniso, rows, sums);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 2;
+  const int nout = 3 + 3 * (1 + ngroups);
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  CUDA_TRY(cudaMemcpy(out, sums, sizeof(double) * nout, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int64_t gpbdev_vecchia_launch_count(gpbdev_vecchia_t h) { return h ? h->launches : 0; }
 int gpbdev_vecchia_knn_replayed(gpbdev_vecchia_t h) { return h ? h->knn_replayed : 0; }
 

@@ -2,7 +2,8 @@
 //
 // vecchia_factor.cuh keeps one matrix row per lane in registers and is specialised on <= 30 neighbours (the headline
 // configuration). This kernel serves what does not fit that layout, with the matrix in shared memory and runtime sizes:
-//   * models with 30 < num_neighbors <= 60 (same modes NLL / STORE / GRAD, same 9 sums, same stored factor layout);
+//   * models with 30 < num_neighbors <= 60 (same modes NLL / STORE / GRAD, same 9 sums, same stored factor layout; BIG_GRAD_ANISO is
+//     MODE_GRAD_ANISO of vecchia_factor.cuh with its kAnisoAcc sums);
 //   * prediction (MODE_PRED): CalcPredVecchiaObservedFirstOrder with CondObsOnly = true (src/GPBoost/Vecchia_utils.cpp:1701-2100;
 //     the reference predicts with 2 x num_neighbors neighbours, re_model_template.h:299): for a prediction point p with observed
 //     neighbours N(p):  A_p = Sigma_NN^-1 Sigma_pN (:1960),  D_p = v - A_p . Sigma_pN (:1925-1931, :1969),  mean_p = A_p y_N (:2061),
@@ -26,7 +27,7 @@ namespace gpb {
 
 constexpr int kBigMaxNeighbors = 60;
 constexpr int kBigLd = 65;  // row stride (doubles) of the shared matrices: 64 + 1, conflict-free for lane = row and lane = column
-enum BigMode : int { BIG_NLL = 0, BIG_STORE = 1, BIG_GRAD = 2, BIG_PRED = 3 };
+enum BigMode : int { BIG_NLL = 0, BIG_STORE = 1, BIG_GRAD = 2, BIG_PRED = 3, BIG_GRAD_ANISO = 4 };
 
 struct BigArgs {
   const double* coords;   // observed points, n_obs x d row-major, Vecchia order
@@ -45,13 +46,14 @@ struct BigArgs {
 };
 
 static inline size_t big_smem_bytes(int mode, int warps, int d) {
-  const size_t per_warp = (size_t)(mode == BIG_GRAD ? 2 : 1) * 64 * kBigLd + 64 * d + 4 * 64;
+  const size_t per_warp = (size_t)(mode == BIG_GRAD || mode == BIG_GRAD_ANISO ? 2 : 1) * 64 * kBigLd + 64 * d + 4 * 64;
   return per_warp * warps * sizeof(double);
 }
 
 template <int COV, int MODE>
 __global__ void __launch_bounds__(128) vecchia_big_kernel(const BigArgs p) {
-  constexpr bool GRAD = MODE == BIG_GRAD;
+  constexpr bool ANISO = MODE == BIG_GRAD_ANISO;
+  constexpr bool GRAD = MODE == BIG_GRAD || ANISO;
   extern __shared__ __align__(16) double big_smem[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, nwib = blockDim.x >> 5;
   const int d = p.d, m = p.m;
@@ -67,6 +69,7 @@ __global__ void __launch_bounds__(128) vecchia_big_kernel(const BigArgs p) {
   double acc[kNumAcc];
 #pragma unroll
   for (int k = 0; k < kNumAcc; ++k) acc[k] = 0.;
+  double acc_an[3] = {0., 0., 0.};  // BIG_GRAD_ANISO: the sums of parameter `lane` (vecchia_factor.cuh, kAnisoAcc)
 
   for (int64_t i = p.row_begin + gwarp; i < p.row_end; i += nwarps) {
     // ---- gather: neighbours (valid entries of a row are a prefix), own location, responses into row q+1
@@ -94,7 +97,7 @@ __global__ void __launch_bounds__(128) vecchia_big_kernel(const BigArgs p) {
         double g = 0.;
         const double val = cov_eval<COV, GRAD>(sqrt(d2), var, range, g);
         S[r * kBigLd + c] = val;
-        if (GRAD) G[r * kBigLd + c] = g;
+        if (GRAD) G[r * kBigLd + c] = ANISO ? (d2 > 0. ? g / d2 : 0.) : g;  // ANISO: g / r^2, split by coordinate share below
       }
     }
     for (int r = lane; r <= q; r += 32) {
@@ -161,17 +164,43 @@ __global__ void __launch_bounds__(128) vecchia_big_kernel(const BigArgs p) {
       for (int c = lane; c <= q; c += 32) { xa[c] = c < q ? -xa[c] : 1.; if (c == q) xw[c] = 0.; }
       __syncwarp();
       double bgb = 0., bgw = 0.;
-      for (int r = 1; r <= q; ++r) {
-        const double br = xa[r], wr = xw[r];
-        for (int c = lane; c < r; c += 32) {
-          const double g = G[r * kBigLd + c];
-          bgb += g * (br * xa[c]);
-          bgw += g * (br * xw[c] + xa[c] * wr);
+      if (ANISO) {
+        const int ng = g_aniso_ngroups;
+        for (int cg = 0; cg < ng; ++cg) {
+          const unsigned mask = g_aniso_mask[cg];
+          double cgb = 0., cgw = 0.;
+          for (int r = 1; r <= q; ++r) {
+            const double br = xa[r], wr = xw[r];
+            for (int c = lane; c < r; c += 32) {
+              const double gq = G[r * kBigLd + c];
+              const double g = gq != 0. ? gq * masked_d2(pts + r * d, pts + c * d, d, mask) : 0.;
+              cgb += g * (br * xa[c]);
+              cgw += g * (br * xw[c] + xa[c] * wr);
+            }
+          }
+          cgb = 2. * warp_sum(cgb);
+          cgw = warp_sum(cgw);
+          if (lane == cg + 1) { bgb = cgb; bgw = cgw; }
         }
+        const double u = By * Dinv_i;
+        const double dDk = lane == 0 ? var - aa - (p.diag_obs - Di) : bgb;
+        const double ukk = lane == 0 ? -aw : -bgw;
+        acc_an[0] += ukk * u;
+        acc_an[1] += u * u * dDk;
+        acc_an[2] += dDk * Dinv_i;
+      } else {
+        for (int r = 1; r <= q; ++r) {
+          const double br = xa[r], wr = xw[r];
+          for (int c = lane; c < r; c += 32) {
+            const double g = G[r * kBigLd + c];
+            bgb += g * (br * xa[c]);
+            bgw += g * (br * xw[c] + xa[c] * wr);
+          }
+        }
+        bgb = 2. * warp_sum(bgb);
+        bgw = warp_sum(bgw);
       }
-      bgb = 2. * warp_sum(bgb);
-      bgw = warp_sum(bgw);
-      if (lane == 0) {
+      if (!ANISO && lane == 0) {
         const double u = By * Dinv_i;
         const double dD0 = var - aa - (p.diag_obs - Di);  // A.s = diag_obs - D (Vecchia_utils.cpp:1623)
         const double dD1 = bgb;
@@ -185,7 +214,13 @@ __global__ void __launch_bounds__(128) vecchia_big_kernel(const BigArgs p) {
     }
     __syncwarp();
   }
-  if (MODE != BIG_PRED && lane == 0) {
+  if (ANISO) {
+    double* row = p.partials + gwarp * kAnisoAcc;
+    if (lane == 0)
+      for (int k = 0; k < 3; ++k) row[k] = acc[k];
+    if (lane <= kMaxAnisoGroups)
+      for (int k = 0; k < 3; ++k) row[3 + 3 * lane + k] = acc_an[k];
+  } else if (MODE != BIG_PRED && lane == 0) {
 #pragma unroll
     for (int k = 0; k < kNumAcc; ++k) p.partials[gwarp * kNumAcc + k] = acc[k];
   }

@@ -45,7 +45,12 @@ enum CovType : int { COV_EXPONENTIAL = 0, COV_MATERN15 = 1, COV_MATERN25 = 2, CO
 // MODE_STORE_GRAD2: the Gaussian (nugget) model's MODE_STORE plus the derivatives of the factor w.r.t. log(var) AND log(range)
 // on the transformed scale, what CalcCovFactorGradientVecchia leaves in B_grad[0..1], D_grad[0..1] — the Fisher information of
 // the covariance parameters (re_model_template.h:10145-10230) applies them to a block of probe vectors.
-enum FactorMode : int { MODE_NLL = 0, MODE_STORE = 1, MODE_GRAD = 2, MODE_STORE_GRAD = 3, MODE_STORE_GRAD2 = 4 };
+// MODE_GRAD_ANISO: the gradient of an anisotropic kernel (ARD / space-time) evaluated on scaled coordinates at range 1: one
+// log-range derivative per coordinate group c instead of one in total. With r^2 the squared scaled distance of a pair and S_c the
+// part of r^2 from the coordinates of group c, dk/dlog(lambda_c) = (dk/dlog(lambda))_iso(r) * S_c / r^2 (0 at r = 0): every pair's
+// isotropic derivative is computed once, as in MODE_GRAD, and split by coordinate share inside the adjoint contractions.
+// Sums go to a kAnisoAcc-wide partial row (see there); the coordinate groups are g_aniso_ngroups / g_aniso_mask.
+enum FactorMode : int { MODE_NLL = 0, MODE_STORE = 1, MODE_GRAD = 2, MODE_STORE_GRAD = 3, MODE_STORE_GRAD2 = 4, MODE_GRAD_ANISO = 5 };
 
 #ifndef GPB_NLL_BLOCKS
 #define GPB_NLL_BLOCKS 5
@@ -59,6 +64,10 @@ constexpr int kMaxNeighbors = 30;  // q + 2 rows must fit one warp
 // per-warp accumulators: 0 sum (By)^2/D  1 sum log D  2 #non-positive D
 //   gradient mode: 3,4 sum u_k u   5,6 sum u^2 dD_k   7,8 sum dD_k / D   (k = 0 variance, 1 range)
 constexpr int kNumAcc = 9;
+// MODE_GRAD_ANISO per-warp sums: 0..2 as above, then for k = 0 (variance) and k = 1..C (range of coordinate group k - 1)
+// 3 + 3k: sum u_k u   4 + 3k: sum u^2 dD_k   5 + 3k: sum dD_k / D. Lane k of the warp owns the three sums of parameter k.
+constexpr int kMaxAnisoGroups = 16;
+constexpr int kAnisoAcc = 3 + 3 * (1 + kMaxAnisoGroups);
 
 struct FactorArgs {
   const double* coords;   // n x d row-major, Vecchia order
@@ -88,6 +97,21 @@ __device__ double* g_factor_dD = nullptr;
 // MODE_STORE_GRAD2 only: d A_i / d log(var) (n x m) and d D_i / d log(var) (n); the range pair goes to g_factor_dA / g_factor_dD
 __device__ double* g_factor_dA0 = nullptr;
 __device__ double* g_factor_dD0 = nullptr;
+// MODE_GRAD_ANISO (and BIG_GRAD_ANISO): number of coordinate groups and, per group, the bit mask of its coordinates
+__constant__ int g_aniso_ngroups;
+__constant__ unsigned g_aniso_mask[kMaxAnisoGroups];
+
+// squared distance of points a and b (rows of pts, stride dim) restricted to the coordinates in mask
+__device__ __forceinline__ double masked_d2(const double* pa, const double* pb, int dim, unsigned mask) {
+  double s = 0.;
+  for (int k = 0; k < dim; ++k) {
+    if ((mask >> k) & 1u) {
+      const double df = pa[k] - pb[k];
+      s = fma(df, df, s);
+    }
+  }
+  return s;
+}
 
 // exp(ax) for ax <= 0 (clamped at -700): round-to-nearest range reduction by the 1.5*2^52 trick, degree-13 Taylor
 // polynomial on |r| <= ln2/2 (truncation error 4e-18), scaling by an exponent-field add. No special-case paths and the
@@ -152,9 +176,12 @@ __device__ __forceinline__ double warp_sum(double x) {
 
 template <int COV, int MODE, int DIM, int MT>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32,
-                                  (MODE == MODE_GRAD || MODE == MODE_STORE_GRAD || MODE == MODE_STORE_GRAD2) ? GPB_GRAD_BLOCKS : GPB_NLL_BLOCKS)
+                                  MODE == MODE_GRAD_ANISO ? 2  // the per-group contractions need more registers than three CTAs leave
+                                  : (MODE == MODE_GRAD || MODE == MODE_STORE_GRAD || MODE == MODE_STORE_GRAD2) ? GPB_GRAD_BLOCKS
+                                                                                                               : GPB_NLL_BLOCKS)
 vecchia_factor_kernel(const FactorArgs p) {
-  constexpr bool GRAD = (MODE == MODE_GRAD);
+  constexpr bool ANISO = (MODE == MODE_GRAD_ANISO);
+  constexpr bool GRAD = (MODE == MODE_GRAD) || ANISO;
   constexpr bool DSTORE = (MODE == MODE_STORE_GRAD) || (MODE == MODE_STORE_GRAD2);  // the range derivative is stored
   constexpr bool GPAIR = GRAD || DSTORE;  // the range-derivative pair values are kept
   constexpr bool SOLVE = (MODE != MODE_NLL);
@@ -180,6 +207,7 @@ vecchia_factor_kernel(const FactorArgs p) {
   double acc[kNumAcc];
 #pragma unroll
   for (int k = 0; k < kNumAcc; ++k) acc[k] = 0.;
+  double acc_an[3] = {0., 0., 0.};  // MODE_GRAD_ANISO: the sums of parameter `lane`
 
   // slot -> source observation of row ii (or -1 for a dummy slot)
   auto slot_src = [&](int64_t ii) -> int64_t {
@@ -252,6 +280,7 @@ vecchia_factor_kernel(const FactorArgs p) {
       const double dist = d2 * rsqrt_fast(d2 + 1e-300);
       double g = 0.;
       double val = cov_eval<COV, GPAIR>(dist, var, range, g);
+      if (ANISO) g = d2 > 0. ? g / d2 : 0.;  // split later by coordinate share: g_c = g S_c / r^2
       if (!full) {
         const bool both = real && ((real_mask >> o) & 1u);
         val = both ? val : 0.;
@@ -415,25 +444,55 @@ vecchia_factor_kernel(const FactorArgs p) {
         // adjoint contractions over this lane's pairs: b^T G b and b^T G w~ (G symmetric, zero diagonal)
         double bgb = 0., bgw = 0.;
         const double bl = xb[lane], wl = xw[lane];
+        if (ANISO) {
+          // per coordinate group c: the same contractions with g_c = (g / r^2) S_c; lane c + 1 keeps group c's results
+          const int ng = g_aniso_ngroups;
+          for (int c = 0; c < ng; ++c) {
+            const unsigned mask = g_aniso_mask[c];
+            double cgb = 0., cgw = 0.;
 #pragma unroll
-        for (int t = 1; t <= NT; ++t) {
-          int o = lane + t;
-          if (o >= P) o -= P;
-          o = lane < P ? o : 0;
-          const double g = gpair[t - 1];  // 0 for padded / inactive pairs
-          const double bo = xb[o], wo = xw[o];
-          bgb += g * (bl * bo);
-          bgw += g * (bl * wo + bo * wl);
+            for (int t = 1; t <= NT; ++t) {
+              int o = lane + t;
+              if (o >= P) o -= P;
+              o = lane < P ? o : 0;
+              const double gq = gpair[t - 1];  // g / r^2; 0 for padded / inactive / coincident pairs
+              const double gc = gq != 0. ? gq * masked_d2(pts + lane * dim, pts + o * dim, dim, mask) : 0.;
+              const double bo = xb[o], wo = xw[o];
+              cgb += gc * (bl * bo);
+              cgw += gc * (bl * wo + bo * wl);
+            }
+            cgb = 2. * warp_sum(cgb);
+            cgw = warp_sum(cgw);
+            if (lane == c + 1) { bgb = cgb; bgw = cgw; }
+          }
+        } else {
+#pragma unroll
+          for (int t = 1; t <= NT; ++t) {
+            int o = lane + t;
+            if (o >= P) o -= P;
+            o = lane < P ? o : 0;
+            const double g = gpair[t - 1];  // 0 for padded / inactive pairs
+            const double bo = xb[o], wo = xw[o];
+            bgb += g * (bl * bo);
+            bgw += g * (bl * wo + bo * wl);
+          }
+          bgb = 2. * warp_sum(bgb);
+          bgw = warp_sum(bgw);
         }
-        bgb = 2. * warp_sum(bgb);
-        bgw = warp_sum(bgw);
         // variance parameter (dSigma~ = Sigma~ without nugget): dD_0 = v - A.A - A.s ; (dB_0 y)_i = -A.w
         // A.s = 1 + v - D  (Vecchia_utils.cpp:1623)
         double aa = (lane < q) ? xa * xa : 0.;
         double aw = (lane < q) ? xa * xwv : 0.;
         aa = warp_sum(aa);
         aw = warp_sum(aw);
-        if (lane == 0) {
+        if (ANISO) {
+          const double u = By * Dinv_i;
+          const double dDk = lane == 0 ? var - aa - (1. + var - Di) : bgb;
+          const double ukk = lane == 0 ? -aw : -bgw;
+          acc_an[0] += ukk * u;
+          acc_an[1] += u * u * dDk;
+          acc_an[2] += dDk * Dinv_i;
+        } else if (lane == 0) {
           const double u = By * Dinv_i;  // (D^-1 B y)_i
           const double dD0 = var - aa - (1. + var - Di);
           const double dD1 = bgb;
@@ -450,7 +509,13 @@ vecchia_factor_kernel(const FactorArgs p) {
     }
     __syncwarp();
   }
-  if (lane == 0) {
+  if (ANISO) {
+    double* row = p.partials + gwarp * kAnisoAcc;
+    if (lane == 0)
+      for (int k = 0; k < 3; ++k) row[k] = acc[k];
+    if (lane <= kMaxAnisoGroups)
+      for (int k = 0; k < 3; ++k) row[3 + 3 * lane + k] = acc_an[k];
+  } else if (lane == 0) {
 #pragma unroll
     for (int k = 0; k < kNumAcc; ++k) p.partials[gwarp * kNumAcc + k] = acc[k];
   }

@@ -283,6 +283,9 @@ int LGBM_BoosterCreate(const DatasetHandle train_data, const char* parameters, B
 int LGBM_GPBoosterCreate(const DatasetHandle train_data, const char* parameters, const REModelHandle re_model, BoosterHandle* out) {
   API_BEGIN();
   if (re_model == nullptr) throw std::runtime_error("LGBM_GPBoosterCreate: re_model is null");
+  if (reinterpret_cast<gpb200::REModel*>(re_model)->IsAnisotropic())
+    throw std::runtime_error("A GP model with an anisotropic covariance function (matern_ard, gaussian_ard, matern_space_time) cannot be "
+                             "used in the GPBoost algorithm by the CUDA engine");
   *out = new gpb200::Booster(reinterpret_cast<const gpb200::Dataset*>(train_data), parameters, reinterpret_cast<gpb200::REModel*>(re_model));
   API_END();
 }
@@ -645,6 +648,12 @@ int GPB200_CalcGradient(REModelHandle handle, double* y_inout) {
 int GPB200_GetNumLikelihoodEvals(REModelHandle handle, int64_t* out) {
   API_BEGIN();
   *out = M(handle)->NumLikelihoodEvals();
+  API_END();
+}
+
+int GPB200_GetNumNeighborSearches(REModelHandle handle, int* out) {
+  API_BEGIN();
+  *out = (int)M(handle)->NumNeighborSearches();
   API_END();
 }
 

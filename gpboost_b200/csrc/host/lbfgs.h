@@ -84,6 +84,11 @@ struct LbfgsParams {
 using LbfgsObjective = std::function<double(const std::vector<double>&, std::vector<double>*, bool)>;
 using LbfgsMaxStep = std::function<double(const std::vector<double>& neg_dir)>;
 using LbfgsHook = std::function<void(bool commit)>;  // commit=true: accept profiled-out state; false: roll back
+// Called after every iteration (after the commit hook) with the reference's iteration counter k - 1 and whether the iteration
+// converged: redetermines state the objective depends on (the Vecchia neighbour sets of anisotropic kernels) when its schedule says
+// so, and returns true when the objective changed. Then the lag-1 value and gradient and the current value and gradient are
+// evaluated again and convergence is tested a second time (LBFGSpp/LBFGS.h:230-260).
+using LbfgsRedetermine = std::function<bool(int num_iter, bool converged)>;
 
 inline double vnorm(const std::vector<double>& v) {
   double s = 0.;
@@ -94,7 +99,7 @@ inline double vnorm(const std::vector<double>& v) {
 // Returns the number of iterations. x in/out, fx out.
 inline int lbfgs_minimize(const LbfgsObjective& f, const LbfgsMaxStep& max_step, const LbfgsHook& hook,
                           const LbfgsParams& par, std::vector<double>* x_io, double* fx_out, LbfgsMemory* mem,
-                          bool reuse_memory) {
+                          bool reuse_memory, const LbfgsRedetermine& redetermine = nullptr) {
   std::vector<double>& x = *x_io;
   const int n = (int)x.size();
   std::vector<double> grad(n), gradp(n), xp(n), drt(n), sv(n), yv(n), negd(n);
@@ -152,8 +157,19 @@ inline int lbfgs_minimize(const LbfgsObjective& f, const LbfgsMaxStep& max_step,
     bool converged = false;
     if (gnorm <= 1e-20 || gnorm <= 1e-20 * vnorm(x)) converged = true;
     if (k >= 1 && (fx_prev - fx) <= par.delta * std::max(std::fabs(fx_prev), 1.)) converged = true;
-    if (par.max_iterations != 0 && k >= par.max_iterations) converged = true;
+    const bool converged_maxit = par.max_iterations != 0 && k >= par.max_iterations;
+    if (converged_maxit) converged = true;
     hook(true);
+    if (redetermine && redetermine(k - 1, converged)) {
+      fx_prev = f(xp, &gradp, false);
+      fx = f(x, &grad, false);
+      if (converged && !converged_maxit) {
+        converged = false;
+        gnorm = vnorm(grad);
+        if (gnorm <= 1e-20 || gnorm <= 1e-20 * vnorm(x)) converged = true;
+        if (k >= 1 && (fx_prev - fx) <= par.delta * std::max(std::fabs(fx_prev), 1.)) converged = true;
+      }
+    }
     if (converged) { *fx_out = fx; return k; }
     for (int i = 0; i < n; ++i) { sv[i] = x[i] - xp[i]; yv[i] = grad[i] - gradp[i]; }
     double sy = 0., yy = 0.;

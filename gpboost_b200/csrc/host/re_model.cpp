@@ -30,6 +30,20 @@ void GrpCheck(int rc) {
   if (rc != 0) Fatal(std::string(gpbdev_grouped_last_error()));
 }
 
+// CalculateMedianPartiallySortInput (utils.h), then the mean when the median is below 1e-10 (cov_fcts.h:1510-1513)
+double MedianOrMean(std::vector<double>* v) {
+  std::vector<double>& dists = *v;
+  const size_t pos_med = dists.size() / 2;
+  std::nth_element(dists.begin(), dists.begin() + pos_med, dists.end());
+  double med = dists[pos_med];
+  if (dists.size() % 2 == 0) {
+    std::nth_element(dists.begin(), dists.begin() + pos_med - 1, dists.end());
+    med = (med + dists[pos_med - 1]) / 2.;
+  }
+  if (med < 1e-10) med = std::accumulate(dists.begin(), dists.end(), 0.) / dists.size();
+  return med;
+}
+
 bool NearlyEqual(double a, double b) { return std::fabs(a - b) < 1e-10 * std::max({1.0, std::fabs(a), std::fabs(b)}); }
 
 // likelihood aliases: include/GPBoost/likelihoods.h:10255-10280 ("poisson" has none; "hurdle_poisson" names zero_inflated_poisson)
@@ -118,18 +132,41 @@ REModel::REModel(int32_t num_data, const int32_t* cluster_ids_data, const char* 
   cov_fct_ = cov_fct;
   shape_ = cov_fct_shape;
   if (cov_fct_ == "exponential" || cov_fct_ == "Matern") { cov_fct_ = "matern"; shape_ = 0.5; }
+  if (cov_fct_ == "exponential_ard" || cov_fct_ == "Matern_ard") { cov_fct_ = "matern_ard"; shape_ = 0.5; }
+  if (cov_fct_ == "exponential_space_time" || cov_fct_ == "Matern_space_time") { cov_fct_ = "matern_space_time"; shape_ = 0.5; }
   if (cov_fct_ == "Gaussian") cov_fct_ = "gaussian";
-  if (cov_fct_ == "matern") {
+  // anisotropic kernels: the isotropic closed form at unit range on scaled coordinates (cov_fcts.h:935-941)
+  aniso_ = cov_fct_ == "matern_ard" || cov_fct_ == "gaussian_ard" || cov_fct_ == "matern_space_time";
+  if (aniso_) {
+    if (!gauss_)
+      Fatal("Covariance of type '" + cov_fct_ + "' is only supported for likelihood 'gaussian' by the CUDA engine (found '" +
+            likelihood_ + "')");
+    if (gp_approx_ != "vecchia")
+      Fatal("Covariance of type '" + cov_fct_ + "' is only supported with gp_approx = 'vecchia' by the CUDA engine");
+    if (GetRuntime().world_size > 1)
+      Fatal("Covariance of type '" + cov_fct_ + "' is not supported with more than one process by the CUDA engine (fit the model in a "
+            "single process)");
+    if (dim_ > 16) Fatal("Covariance of type '" + cov_fct_ + "' supports at most 16 coordinates in the CUDA engine");
+    if (cov_fct_ == "matern_space_time" && dim_ < 2)
+      Fatal("Covariance of type 'matern_space_time' needs a time coordinate and at least one space coordinate");
+    const bool space_time = cov_fct_ == "matern_space_time";
+    num_aniso_groups_ = space_time ? 2 : dim_;
+    aniso_group_.resize(dim_);
+    for (int k = 0; k < dim_; ++k) aniso_group_[k] = space_time ? (k == 0 ? 0 : 1) : k;
+  }
+  const std::string cov_base = aniso_ ? (cov_fct_ == "gaussian_ard" ? "gaussian" : "matern") : cov_fct_;
+  if (cov_base == "matern") {
     if (NearlyEqual(shape_, 0.5)) cov_id_ = GPBDEV_COV_EXPONENTIAL;
     else if (NearlyEqual(shape_, 1.5)) cov_id_ = GPBDEV_COV_MATERN15;
     else if (NearlyEqual(shape_, 2.5)) cov_id_ = GPBDEV_COV_MATERN25;
     else Fatal("Only Matern smoothness 0.5, 1.5 and 2.5 are supported by the CUDA engine (found " + std::to_string(shape_) + ")");
-  } else if (cov_fct_ == "gaussian") {
+  } else if (cov_base == "gaussian") {
     cov_id_ = GPBDEV_COV_GAUSSIAN;
   } else {
     Fatal("Covariance of type '" + cov_fct_ + "' is not supported by the CUDA engine.");
   }
   num_cov_pars_ = gauss_ ? 3 : 2;  // (nugget,) marginal variance, range
+  if (aniso_) num_cov_pars_ = 2 + num_aniso_groups_;  // nugget, marginal variance, one range per coordinate group
   // ---- GP approximation
   std::memset(laplace_out_, 0, sizeof(laplace_out_));
   if (gp_approx_ == "none") {  // exact GP: dense Gram + Cholesky on the device, original observation order
@@ -148,15 +185,29 @@ REModel::REModel(int32_t num_data, const int32_t* cluster_ids_data, const char* 
   num_neighbors_ = num_neighbors > 0 ? num_neighbors : 20;  // re_model_template.h:288-294
   num_neighbors_pred_ = 2 * num_neighbors_;                  // re_model_template.h:299
   vecchia_ordering_ = vecchia_ordering == nullptr ? "none" : std::string(vecchia_ordering);
-  if (vecchia_ordering_ != "none" && vecchia_ordering_ != "random")
+  const bool time_ordering = vecchia_ordering_ == "time" || vecchia_ordering_ == "time_random_space";
+  if (vecchia_ordering_ != "none" && vecchia_ordering_ != "random" && !time_ordering)
     Fatal("Ordering of type '" + vecchia_ordering_ + "' is not supported for the Veccia approximation ");
+  if (time_ordering && cov_fct_ != "matern_space_time")  // Vecchia_utils.cpp:1174-1176
+    Fatal("'vecchia_ordering' is '" + vecchia_ordering_ + "' but the 'cov_function' is not a space-time covariance function ");
   if (num_neighbors_ > num_data_ - 1) num_neighbors_ = std::max(num_data_ - 1, 1);  // Vecchia_utils.cpp:755-758
   // ---- ordering: data_indices_per_cluster = 0..n-1, shuffled with rng_ for "random" (Vecchia_utils.cpp:1129-1131)
   perm_.resize(num_data_);
   {
     std::vector<int> idx(num_data_);
     std::iota(idx.begin(), idx.end(), 0);
-    if (vecchia_ordering_ == "random") std::shuffle(idx.begin(), idx.end(), rng_);
+    if (vecchia_ordering_ == "random" || vecchia_ordering_ == "time_random_space") std::shuffle(idx.begin(), idx.end(), rng_);
+    if (time_ordering) {
+      // SortIndeces (utils.h:230-238) of the time column in the current order: the same std::sort call, so ties end up where the
+      // reference puts them (Vecchia_utils.cpp:1138-1154)
+      std::vector<double> t(num_data_);
+      for (int32_t i = 0; i < num_data_; ++i) t[i] = gp_coords_data[idx[i]];
+      std::vector<int> order(num_data_);
+      std::iota(order.begin(), order.end(), 0);
+      std::sort(order.begin(), order.end(), [&t](int i1, int i2) { return t[i1] < t[i2]; });
+      std::vector<int> unsorted = idx;
+      for (int32_t i = 0; i < num_data_; ++i) idx[i] = unsorted[order[i]];
+    }
     for (int32_t i = 0; i < num_data_; ++i) perm_[i] = idx[i];
   }
   // coordinates arrive column-major (gp_coords_data[j*num_data+i], Vecchia_utils.cpp:1133-1137); keep them
@@ -172,8 +223,12 @@ REModel::REModel(int32_t num_data, const int32_t* cluster_ids_data, const char* 
     rb = std::min<int64_t>(num_data_, chunk * rt.rank);
     re = std::min<int64_t>(num_data_, rb + chunk);
   }
-  DevCheck(gpbdev_vecchia_create(&engine_, rt.device, num_data_, dim_, num_neighbors_, coords_ordered_.data(), perm_.data(),
-                                 nullptr, rb, re));
+  if (aniso_)  // neighbour sets are searched at the first factorisation, in the space scaled by its parameters (Vecchia_utils.cpp:1184)
+    DevCheck(gpbdev_vecchia_create_unsearched(&engine_, rt.device, num_data_, dim_, num_neighbors_, coords_ordered_.data(), perm_.data(),
+                                              rb, re));
+  else
+    DevCheck(gpbdev_vecchia_create(&engine_, rt.device, num_data_, dim_, num_neighbors_, coords_ordered_.data(), perm_.data(),
+                                   nullptr, rb, re));
   if (rt.world_size > 1 && gauss_ && rt.allreduce_dev != nullptr) {
     // native collective (GPB200_NcclInit): the engine sums its shard results over the ranks on its own stream
     DevCheck(gpbdev_vecchia_set_allreduce(engine_, rt.allreduce_dev, rt.allreduce_ctx));
@@ -267,12 +322,14 @@ void REModel::TransformCovPars(const double* orig, double* trans) const {
   trans[1] = orig[1] / s2;
   for (int k = 2; gmulti_ && k < num_cov_pars_; ++k) trans[k] = orig[k] / s2;
   if (grouped_ || gmulti_) return;  // RECompGroup: only the variance is rescaled (re_comp.h:300-310)
-  if (!(orig[2] > 0.)) Fatal("Check failed: pars[1] > 0.");
-  switch (cov_id_) {
-    case GPBDEV_COV_EXPONENTIAL: trans[2] = 1. / orig[2]; break;
-    case GPBDEV_COV_MATERN15: trans[2] = std::sqrt(3.) / orig[2]; break;
-    case GPBDEV_COV_MATERN25: trans[2] = std::sqrt(5.) / orig[2]; break;
-    default: trans[2] = 1. / (orig[2] * orig[2]); break;
+  for (int k = 2; k < num_cov_pars_; ++k) {  // one range, or one per coordinate group (cov_fcts.h:523-545)
+    if (!(orig[k] > 0.)) Fatal("Check failed: pars[1] > 0.");
+    switch (cov_id_) {
+      case GPBDEV_COV_EXPONENTIAL: trans[k] = 1. / orig[k]; break;
+      case GPBDEV_COV_MATERN15: trans[k] = std::sqrt(3.) / orig[k]; break;
+      case GPBDEV_COV_MATERN25: trans[k] = std::sqrt(5.) / orig[k]; break;
+      default: trans[k] = 1. / (orig[k] * orig[k]); break;
+    }
   }
 }
 
@@ -293,11 +350,13 @@ void REModel::TransformBackCovPars(const double* trans, double* orig) const {
   orig[1] = s2 * trans[1];
   for (int k = 2; gmulti_ && k < num_cov_pars_; ++k) orig[k] = s2 * trans[k];
   if (grouped_ || gmulti_) return;
-  switch (cov_id_) {
-    case GPBDEV_COV_EXPONENTIAL: orig[2] = 1. / trans[2]; break;
-    case GPBDEV_COV_MATERN15: orig[2] = std::sqrt(3.) / trans[2]; break;
-    case GPBDEV_COV_MATERN25: orig[2] = std::sqrt(5.) / trans[2]; break;
-    default: orig[2] = 1. / std::sqrt(trans[2]); break;
+  for (int k = 2; k < num_cov_pars_; ++k) {  // cov_fcts.h:597-619
+    switch (cov_id_) {
+      case GPBDEV_COV_EXPONENTIAL: orig[k] = 1. / trans[k]; break;
+      case GPBDEV_COV_MATERN15: orig[k] = std::sqrt(3.) / trans[k]; break;
+      case GPBDEV_COV_MATERN25: orig[k] = std::sqrt(5.) / trans[k]; break;
+      default: orig[k] = 1. / std::sqrt(trans[k]); break;
+    }
   }
 }
 
@@ -369,7 +428,7 @@ void REModel::FindInitCovPar(const double* y_data, const double* fixed_effects, 
   }
   std::vector<double> dists;
   dists.reserve((size_t)ns * (ns - 1) / 2);
-  for (int i = 0; i < ns - 1; ++i)
+  for (int i = 0; !aniso_ && i < ns - 1; ++i)
     for (int j = i + 1; j < ns; ++j) {
       double s = 0.;
       for (int k = 0; k < dim_; ++k) {
@@ -378,15 +437,12 @@ void REModel::FindInitCovPar(const double* y_data, const double* fixed_effects, 
       }
       dists.push_back(std::sqrt(s));
     }
-  if (dists.empty()) Fatal("Cannot find an initial value for the range parameter");
-  const size_t pos_med = dists.size() / 2;
-  std::nth_element(dists.begin(), dists.begin() + pos_med, dists.end());
-  double med = dists[pos_med];
-  if (dists.size() % 2 == 0) {
-    std::nth_element(dists.begin(), dists.begin() + pos_med - 1, dists.end());
-    med = (med + dists[pos_med - 1]) / 2.;
+  if (aniso_) {
+    FindInitRangesAniso(sample, init_trans + 2);
+    return;
   }
-  if (med < 1e-10) med = std::accumulate(dists.begin(), dists.end(), 0.) / dists.size();
+  if (dists.empty()) Fatal("Cannot find an initial value for the range parameter");
+  double med = MedianOrMean(&dists);
   if (med < 1e-10)
     Fatal("Cannot find an initial value for the range parameter since both the median and the average distances among coordinates are zero ");
   if (cov_fct_ == "matern") {
@@ -395,6 +451,71 @@ void REModel::FindInitCovPar(const double* y_data, const double* fixed_effects, 
     else init_trans[2] = 2. * 5.9 / med;
   } else {
     init_trans[2] = 3. / std::pow(med / 2., 2.);
+  }
+}
+
+// FindInitCovPar for matern_ard / gaussian_ard / matern_space_time (cov_fcts.h:1440-1670) on the ordered coordinates and the sub-sample
+// the isotropic rule draws: per-coordinate median absolute distances (ARD; (k^2 - 1) / (3k) for a coordinate with k <= 10 unique
+// values, an error for a constant one), or separate median time and space distances. Writes the C transformed ranges.
+void REModel::FindInitRangesAniso(const std::vector<int>& sample, double* init_ranges) const {
+  const int n = num_data_, d = dim_, ns = (int)sample.size();
+  const std::string sub = ns < n ? "on a random sub-sample of size 1000 " : "";
+  auto coord = [&](int s, int k) { return coords_ordered_[(size_t)sample[s] * d + k]; };
+  const double mult = shape_ <= 1. ? 2. * 3. : (shape_ <= 2. ? 2. * 4.7 : 2. * 5.9);
+  std::vector<double> dists;
+  dists.reserve((size_t)ns * (ns - 1) / 2);
+  if (cov_fct_ == "matern_space_time") {
+    std::vector<double> dt;
+    dt.reserve(dists.capacity());
+    for (int i = 0; i < ns - 1; ++i)
+      for (int j = i + 1; j < ns; ++j) {
+        double s = 0.;
+        for (int k = 1; k < d; ++k) {
+          const double t = coord(i, k) - coord(j, k);
+          s += t * t;
+        }
+        dists.push_back(std::sqrt(s));
+        dt.push_back(std::fabs(coord(i, 0) - coord(j, 0)));
+      }
+    if (dists.empty()) Fatal("Cannot find an initial value for the range parameter");
+    const double med_space = MedianOrMean(&dists), med_time = MedianOrMean(&dt);
+    if (med_space < 1e-10)
+      Fatal("Cannot find an initial value for the range parameter since both the median and the average distances among coordinates "
+            "are zero " + sub);
+    if (med_time < 1e-10)
+      Fatal("Cannot find an initial value for the temporal range parameter since both the median and the average distances among time "
+            "points are zero " + sub);
+    init_ranges[0] = mult / med_time;
+    init_ranges[1] = mult / med_space;
+    return;
+  }
+  for (int k = 0; k < d; ++k) {
+    // NumberUniqueValues(col, 11) over all observations (utils.h:159-183): only "1", "<= 10" and "more" matter
+    std::vector<double> uniq;
+    for (int32_t i = 0; i < n && (int)uniq.size() <= 11; ++i) {
+      const double v = coords_ordered_[(size_t)i * d + k];
+      if (std::find(uniq.begin(), uniq.end(), v) == uniq.end()) uniq.push_back(v);
+    }
+    const int nu = (int)uniq.size();
+    double med = 0.;
+    bool constant = nu == 1;
+    std::string err_sub = sub;
+    if (constant) {
+      err_sub = "";
+    } else if (nu <= 10) {
+      med = (nu * nu - 1) / 3. / nu;  // mean distance of two random points on {1, ..., nu}
+    } else {
+      dists.clear();
+      for (int i = 0; i < ns - 1; ++i)
+        for (int j = i + 1; j < ns; ++j) dists.push_back(std::fabs(coord(i, k) - coord(j, k)));
+      if (dists.empty()) Fatal("Cannot find an initial value for the range parameter");
+      med = MedianOrMean(&dists);
+      constant = med < 1e-10;
+    }
+    if (constant)
+      Fatal("Cannot find an initial value for the range parameter for the input feature number " + std::to_string(k + 1) +
+            " (counting starts at 1) since this feature is constant " + err_sub);
+    init_ranges[k] = cov_fct_ == "gaussian_ard" ? 3. / std::pow(med / 2., 2.) : mult / med;
   }
 }
 
@@ -423,6 +544,30 @@ void REModel::SetY(const double* y_data, const double* fixed_effects) {
   else if (gmulti_) GrpCheck(gpbdev_grouped_multi_set_y(gmulti_, src));
   else if (dense_) DenseCheck(gpbdev_dense_set_y(dense_, src));
   else DevCheck(gpbdev_vecchia_set_y(engine_, src));
+}
+
+void REModel::AnisoScale(const double* lambda, std::vector<double>* scale) const {
+  scale->resize(dim_);
+  for (int k = 0; k < dim_; ++k) {
+    const double l = lambda[aniso_group_[k]];
+    (*scale)[k] = cov_id_ == GPBDEV_COV_GAUSSIAN ? std::sqrt(l) : l;
+  }
+}
+
+// The neighbour sets live in the space scaled by the parameters they were searched at: a likelihood evaluation searches them at its
+// parameters, a fit at the initial parameters and then on the optimiser's schedule; in between they stay as they are.
+void REModel::AnisoSetRanges(const double* lambda, bool search) {
+  std::vector<double> scale;
+  AnisoScale(lambda, &scale);
+  if (scale != aniso_scale_) {
+    DevCheck(gpbdev_vecchia_set_coord_scale(engine_, scale.data()));
+    aniso_scale_ = scale;
+  }
+  if (search || !nn_determined_) {
+    DevCheck(gpbdev_vecchia_search_neighbors(engine_));
+    nn_determined_ = true;
+    ++num_nn_searches_;
+  }
 }
 
 void REModel::DevicePass(double var, double range, int mode) {
@@ -655,6 +800,9 @@ void REModel::EvalNegLogLikelihood(const double* y_data, const double* cov_pars,
   if (grouped_) GroupedPass(trans[1]);
   else if (gmulti_) GroupedMultiPass(trans.data() + 1);
   else if (dense_) DensePass(trans[1], trans[2]);
+  // an evaluation outside a fit searches the neighbour sets at its own parameters: the reference's value at theta2 is the same
+  // whether the model evaluated theta1 before or not (tests/golden/aniso_golden.json)
+  else if (aniso_) { AnisoSetRanges(trans.data() + 2, true); DevicePass(trans[1], 1., GPBDEV_MODE_NLL); }
   else DevicePass(trans[1], trans[2], GPBDEV_MODE_NLL);
   *negll = NegLLFromSums(trans[0]);
   if (gmulti_) laplace_out_[0] = *negll;
@@ -698,11 +846,12 @@ void REModel::Predict(const double* y_obs, int32_t num_data_pred, double* out_pr
   if (!gauss_) Fatal("Prediction is not supported for likelihood '" + likelihood_ + "' by the CUDA engine yet");
   if (predict_cov_mat) Fatal("Predictive covariance matrices are not supported by the CUDA engine (predict_var gives the variances)");
   if (out_predict == nullptr) Fatal("Check failed: out_predict != nullptr");
-  double trans[3] = {0., 0., 1.};
+  std::vector<double> trans(std::max(3, num_cov_pars_), 0.);
+  trans[2] = 1.;
   if (cov_pars_pred != nullptr) {
     for (int i = 0; i < num_cov_pars_; ++i)
       if (!(cov_pars_pred[i] > 0.)) Fatal("Covariance parameters must be positive");
-    TransformCovPars(cov_pars_pred, trans);
+    TransformCovPars(cov_pars_pred, trans.data());
   } else {
     if (!cov_pars_initialized_) Fatal("Covariance parameters have not been estimated or are not given.");  // re_model.cpp:1119-1121
     for (int i = 0; i < num_cov_pars_; ++i) trans[i] = cov_pars_[i];
@@ -746,7 +895,24 @@ void REModel::Predict(const double* y_obs, int32_t num_data_pred, double* out_pr
     Fatal("Response variable data is not available for making predictions (pass y or fit the model first)");
   }
   std::vector<double> dvar((size_t)num_data_pred);
-  DevCheck(gpbdev_vecchia_predict(engine_, cov_id_, trans[1], trans[2], cp, num_data_pred, num_neighbors_pred_, out_predict, dvar.data()));
+  double range = trans[2];
+  std::vector<double> cp_scaled;
+  if (aniso_) {
+    // the prediction points' neighbours are searched among the observed points in the space scaled by the prediction's parameters
+    // (Vecchia_utils.cpp:1755-1760); the training neighbour sets are not touched
+    std::vector<double> scale;
+    AnisoScale(trans.data() + 2, &scale);
+    if (scale != aniso_scale_) {
+      DevCheck(gpbdev_vecchia_set_coord_scale(engine_, scale.data()));
+      aniso_scale_ = scale;
+    }
+    cp_scaled.resize((size_t)num_data_pred * dim_);
+    for (int32_t i = 0; i < num_data_pred; ++i)
+      for (int k = 0; k < dim_; ++k) cp_scaled[(size_t)i * dim_ + k] = cp[(size_t)i * dim_ + k] * scale[k];
+    cp = cp_scaled.data();
+    range = 1.;
+  }
+  DevCheck(gpbdev_vecchia_predict(engine_, cov_id_, trans[1], range, cp, num_data_pred, num_neighbors_pred_, out_predict, dvar.data()));
   if (Xp != nullptr) {
     for (int c = 0; c < num_covariates_; ++c) {
       const double* Xc = Xp + (size_t)c * num_data_pred;
@@ -765,6 +931,7 @@ std::string REModel::ValidationPredictionUnsupportedReason() const {
     return "the grouped and exact GP models cannot predict in this build yet: set use_gp_model_for_validation=False to validate on the "
            "tree ensemble's scores";
   if (!gauss_) return "prediction is not supported for likelihood '" + likelihood_ + "' by the CUDA engine yet";
+  if (aniso_) return "covariance of type '" + cov_fct_ + "' cannot be used in the GPBoost algorithm by the CUDA engine";
   if (num_covariates_ > 0) return "a GP model with linear regression covariates cannot be used for validation in the GPBoost algorithm";
   return "";
 }
@@ -883,6 +1050,7 @@ void REModel::OptimCovParDevice(const double* y_dev, bool called_in_GPBoost_algo
   std_dev_cov_pars_calculated_ = false;  // re_model.cpp:543, :629
   if (y_dev == nullptr) Fatal("Check failed: y_data != nullptr");
   if (!DevicePathReady()) Fatal("OptimCovParDevice: no device-resident path for this model state (use OptimCovPar)");
+  if (aniso_) Fatal("Covariance of type '" + cov_fct_ + "' cannot be used in the GPBoost algorithm by the CUDA engine");
   num_covariates_ = 0;
   SetYDevice(y_dev);
   OptimCovParCore(called_in_GPBoost_algorithm, reuse_learning_rates_from_previous_call);
@@ -957,6 +1125,50 @@ void REModel::OptimCovParCore(bool called_in_GPBoost_algorithm, bool reuse_learn
     }
     return f;
   };
+  // anisotropic kernels: optimisation variables log(var ratio), log(lambda_1) .. log(lambda_C); the likelihood pass is the isotropic
+  // kernel at range 1 on the coordinates scaled by lambda, the gradient pass has one range derivative per coordinate group
+  const int na = 3 + 3 * (1 + num_aniso_groups_);
+  std::vector<double> aniso_out(aniso_ ? na : 0);
+  LbfgsObjective objective_aniso = [&](const std::vector<double>& x, std::vector<double>* grad, bool speculative) -> double {
+    if (grad != nullptr && have_cached_grad && cached_x == x) {
+      *grad = cached_grad;
+      return cached_f;
+    }
+    std::vector<double> lambda(x.size() - 1);
+    for (size_t k = 1; k < x.size(); ++k) lambda[k - 1] = std::exp(x[k]);
+    const double var = std::exp(x[0]);
+    AnisoSetRanges(lambda.data(), false);
+    const bool with_grad = grad != nullptr || speculative;
+    if (with_grad) {
+      DevCheck(gpbdev_vecchia_eval_grad_aniso(engine_, cov_id_, var, aniso_group_.data(), num_aniso_groups_, aniso_out.data()));
+      for (int k = 0; k < 3; ++k) sums_[k] = aniso_out[k];
+      ++num_ll_evals_;
+    } else {
+      DevicePass(var, 1., GPBDEV_MODE_NLL);
+    }
+    sigma2 = sums_[GPBDEV_SUM_QUAD] / num_data_;  // ProfileOutSigma2
+    const double f = NegLLFromSums(sigma2);
+    have_cached_grad = false;
+    if (with_grad) {
+      cached_grad.assign(x.size(), 0.);
+      for (size_t k = 0; k < x.size(); ++k)  // re_model_template.h:2002-2004, one entry per parameter
+        cached_grad[k] = (aniso_out[3 + 3 * k] - 0.5 * aniso_out[4 + 3 * k]) / sigma2 + 0.5 * aniso_out[5 + 3 * k];
+      cached_x = x; cached_f = f; have_cached_grad = true;
+      if (grad != nullptr) *grad = cached_grad;
+    }
+    return f;
+  };
+  // neighbour sets redetermined in the space scaled at the current parameters after iteration k when k - 1 is 0 or 2^j - 1, and on
+  // convergence (ShouldRedetermineNearestNeighborsVecchiaInducingPointsFITC, re_model_template.h:5382-5404); the reference then
+  // evaluates the lag-1 and the current objective again, which the optimiser does when this returns true
+  LbfgsRedetermine redetermine = [&](int num_iter, bool converged) -> bool {
+    if (!(((num_iter + 1) & num_iter) == 0 || num_iter == 0 || converged)) return false;
+    // the last evaluation was at the accepted point: the engine's coordinates are scaled by its parameters
+    DevCheck(gpbdev_vecchia_search_neighbors(engine_));
+    ++num_nn_searches_;
+    have_cached_grad = false;
+    return true;
+  };
   LbfgsMaxStep max_step = [&](const std::vector<double>& neg_dir) {  // re_model_template.h:5413-5421
     double mx = 0.;
     for (double v : neg_dir) mx = std::max(mx, std::fabs(v));
@@ -973,12 +1185,15 @@ void REModel::OptimCovParCore(bool called_in_GPBoost_algorithm, bool reuse_learn
   par.m = m_lbfgs_;
   par.initial_step_factor = lr_cov_init_;
   std::vector<double> x = {std::log(cov_pars_[1])};
-  if (gmulti_)
+  if (aniso_) {
+    for (int k = 2; k < num_cov_pars_; ++k) x.push_back(std::log(cov_pars_[k]));
+    AnisoSetRanges(cov_pars_.data() + 2, true);  // redetermined at the initial parameters (re_model_template.h:1376-1379)
+  } else if (gmulti_)
     for (int k = 2; k < num_cov_pars_; ++k) x.push_back(std::log(cov_pars_[k]));
   else if (!grouped_) x.push_back(std::log(cov_pars_[2]));
   double fx = 0.;
-  num_it_ = lbfgs_minimize(grouped_ ? objective_grouped : gmulti_ ? objective_gmulti : objective, max_step, hook, par, &x, &fx, &lbfgs_mem_,
-                           reuse_mem);
+  num_it_ = lbfgs_minimize(grouped_ ? objective_grouped : gmulti_ ? objective_gmulti : aniso_ ? objective_aniso : objective, max_step, hook,
+                           par, &x, &fx, &lbfgs_mem_, reuse_mem, aniso_ ? redetermine : LbfgsRedetermine());
   cov_pars_[0] = sigma2;
   for (size_t k = 0; k < x.size(); ++k) cov_pars_[k + 1] = std::exp(x[k]);
   for (double v : cov_pars_)
@@ -989,6 +1204,7 @@ void REModel::OptimCovParCore(bool called_in_GPBoost_algorithm, bool reuse_learn
 
 void REModel::CalcGradient(double* y, const double* fixed_effects, bool /*calc_cov_factor*/) {
   if (!gauss_) Fatal("CalcGradient for likelihood '" + likelihood_ + "' is not built on the device yet");
+  if (aniso_) Fatal("Covariance of type '" + cov_fct_ + "' cannot be used in the GPBoost algorithm by the CUDA engine");
   if (y == nullptr) Fatal("Check failed: y != nullptr");
   InitializeCovParsIfNotDefined(y, fixed_effects);
   // re_model_template.h:3298-3321: SetY(y); y_aux = Psi^-1 y / sigma^2; written back on y.
@@ -1024,6 +1240,7 @@ void REModel::CalcGradient(double* y, const double* fixed_effects, bool /*calc_c
 
 void REModel::CalcGradientDevice(double* y_dev, bool response_is_current) {
   if (!gauss_) Fatal("CalcGradient for likelihood '" + likelihood_ + "' is not built on the device yet");
+  if (aniso_) Fatal("Covariance of type '" + cov_fct_ + "' cannot be used in the GPBoost algorithm by the CUDA engine");
   if (y_dev == nullptr) Fatal("Check failed: y != nullptr");
   if (!DevicePathReady()) Fatal("CalcGradientDevice: no device-resident path for this model state (use CalcGradient)");
   if (grouped_) {
@@ -1181,6 +1398,8 @@ void REModel::OptimLinRegrCoefCovPar(const double* y_data, const double* covaria
     OptimCovPar(y_data, fixed_effects, false, false);
     return;
   }
+  if (aniso_)
+    Fatal("Linear regression covariates are not supported for covariance of type '" + cov_fct_ + "' by the CUDA engine");
   if (engine_ == nullptr || !gauss_)
     Fatal("Linear regression covariates are only supported for the Gaussian Vecchia GP model by the CUDA engine "
           "(not for grouped random effects, exact GPs ('gp_approx = none') or likelihood '" + likelihood_ + "')");
@@ -1283,6 +1502,7 @@ std::string REModel::StdDevCovParsUnsupportedReason() const {
   const std::string pre = "Standard errors of covariance parameters are not available in the CUDA engine ";
   if (!gauss_) return pre + "for likelihood '" + likelihood_ + "' (only for 'gaussian')";
   if (engine_ == nullptr) return pre + "for this model (only for a Gaussian process with gp_approx = 'vecchia')";
+  if (aniso_) return pre + "for covariance of type '" + cov_fct_ + "'";
   const Runtime& rt = GetRuntime();
   if (rt.world_size > 1) return pre + "for a model whose observations are sharded over several GPUs";
   if (num_neighbors_ > 30) return pre + "for num_neighbors > 30 (found " + std::to_string(num_neighbors_) + ")";

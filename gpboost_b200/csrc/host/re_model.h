@@ -101,6 +101,11 @@ class REModel {
   const std::string& LikelihoodName() const { return likelihood_; }
   const std::string& OptimizerCovPars() const { return optimizer_; }
   int64_t NumLikelihoodEvals() const { return num_ll_evals_; }
+  // searches of the Vecchia neighbour sets in the scaled space of an anisotropic kernel (0 for every other model)
+  int64_t NumNeighborSearches() const { return num_nn_searches_; }
+  // matern_ard, gaussian_ard or matern_space_time: the covariance is the isotropic closed form at unit range on coordinates scaled
+  // column by column by the covariance parameters
+  bool IsAnisotropic() const { return aniso_; }
   gpbdev_vecchia_t Engine() const { return engine_; }
   bool IsGrouped() const { return grouped_ != nullptr || gmulti_ != nullptr; }
   // transformed <-> original scale (cov_fcts.h:485-623)
@@ -121,6 +126,21 @@ class REModel {
   // y - offset - X coef_ becomes the engine's response; sums_ QUAD / LOGDET / NBAD belong to the residual
   void ProfileOutCoef(double var, double range);
   void InitCoefFromIidModel(const double* y_data, const double* fixed_effects);
+  // anisotropic kernels (matern_ard, gaussian_ard, matern_space_time): C = num_aniso_groups_ ranges on the transformed scale,
+  // lambda_c = c / rho_c (matern, c = 1, sqrt 3, sqrt 5) or 1 / rho_c^2 (gaussian_ard); coordinate k belongs to group
+  // aniso_group_[k] (ARD: k; space-time: time 0, space 1) and is multiplied by lambda or sqrt(lambda) (ScaleCoordinates,
+  // cov_fcts.h:280-313)
+  bool aniso_ = false;
+  int num_aniso_groups_ = 0;
+  std::vector<int32_t> aniso_group_;
+  std::vector<double> aniso_scale_;     // factors the engine's coordinates are scaled by now (empty: not scaled yet)
+  bool nn_determined_ = false;          // the neighbour sets have been searched at least once
+  int64_t num_nn_searches_ = 0;
+  void AnisoScale(const double* lambda, std::vector<double>* scale) const;
+  // scales the engine's coordinates by the transformed ranges lambda (C values); searches the neighbour sets there when
+  // `search` or when they have never been searched
+  void AnisoSetRanges(const double* lambda, bool search);
+  void FindInitRangesAniso(const std::vector<int>& sample, double* init_ranges) const;
 
   int32_t num_data_ = 0;
   int dim_ = 0;

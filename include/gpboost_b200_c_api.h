@@ -148,6 +148,9 @@ GPB200_EXPORT int GPB200_NcclFinalize(void);
 GPB200_EXPORT int GPB200_CalcGradient(REModelHandle handle, double* y_inout);
 /* number of device likelihood passes so far */
 GPB200_EXPORT int GPB200_GetNumLikelihoodEvals(REModelHandle handle, int64_t* out);
+/* anisotropic covariance functions (matern_ard, gaussian_ard, matern_space_time): number of searches of the Vecchia neighbour sets in
+ * the scaled space so far (lazily at the first factorisation, at the start of a fit and on the optimiser's schedule); 0 otherwise */
+GPB200_EXPORT int GPB200_GetNumNeighborSearches(REModelHandle handle, int* out);
 /* non-Gaussian likelihoods (Laplace approximation), after GPB_EvalNegLogLikelihood: out6 = {negll, Newton iterations of the
  * mode finding, CG iterations, SLQ iterations, log det(Sigma W + I), objective at the mode}; and the posterior mode of the
  * latent process in the original data order (likelihoods.h: mode_, num_it_mode_finding_) */

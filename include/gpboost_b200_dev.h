@@ -54,6 +54,25 @@ GPBDEV_EXPORT int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64
                                         const double* coords_ordered, const int32_t* perm,
                                         const int32_t* nn, int64_t row_begin, int64_t row_end);
 GPBDEV_EXPORT int gpbdev_vecchia_free(gpbdev_vecchia_t h);
+/* The same engine without neighbour sets: for anisotropic kernels, whose sets are searched in the space scaled by covariance
+ * parameters (gpbdev_vecchia_search_neighbors), never at creation. Every pass fails until the first search. */
+GPBDEV_EXPORT int gpbdev_vecchia_create_unsearched(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m,
+                                                   const double* coords_ordered, const int32_t* perm, int64_t row_begin,
+                                                   int64_t row_end);
+/* Anisotropic kernels (matern_ard, gaussian_ard, matern_space_time) are the isotropic closed forms at unit range on coordinates scaled
+ * column by column (ScaleCoordinates, cov_fcts.h:280-313). set_coord_scale: the engine's coordinates become the coordinates given at
+ * creation times scale[k] in column k (d positive factors, one rounded multiply per entry, so a host computing coords[i][k] * scale[k]
+ * gets the same bits); every pass, prediction set and search afterwards sees the scaled coordinates, evaluated with range = 1.
+ * search_neighbors: reruns the device neighbour search on the current (scaled) coordinates and replaces the sets; the stored factor,
+ * the CSC view and the Laplace state are dropped, and prediction sets created before must be rebuilt by their owner.
+ * eval_grad_aniso: the Gaussian likelihood's gradient pass at transformed var and range 1 with one log-range derivative per coordinate
+ * group (group_of_coord: d ids in [0, ngroups), 1 <= ngroups <= 16). out (3 + 3 (1 + ngroups) doubles) = QUAD, LOGDET, NBAD, then
+ * for parameter k = 0 (variance), 1..ngroups (range of group k - 1): sum u_k u, sum u^2 dD_k, sum dD_k / D as GPBDEV_SUM_UKU0 /
+ * UDU0 / TR0 for the isotropic gradient. num_neighbors <= 60. */
+GPBDEV_EXPORT int gpbdev_vecchia_set_coord_scale(gpbdev_vecchia_t h, const double* scale);
+GPBDEV_EXPORT int gpbdev_vecchia_search_neighbors(gpbdev_vecchia_t h);
+GPBDEV_EXPORT int gpbdev_vecchia_eval_grad_aniso(gpbdev_vecchia_t h, int cov_type, double var, const int32_t* group_of_coord,
+                                                 int ngroups, double* out);
 
 /* copy the neighbour sets back (n x m int32, -1 padded) — parity tests */
 GPBDEV_EXPORT int gpbdev_vecchia_get_nn(gpbdev_vecchia_t h, int32_t* nn_host);
