@@ -116,7 +116,9 @@ __global__ void diag_kernel(int G, const int32_t* __restrict__ comp, const doubl
   }
 }
 
-// out[c] = sum_{i in [r0, r1)} A[i t + c] B[i t + c]: one block per column, contiguous slice per thread, fixed-order tree
+// out[c] = sum_{i in [r0, r1)} A[i t + c] B[i t + c] (kAbs: sum of |A[i t + c]|, B unused): one block per column, contiguous slice
+// per thread, fixed-order tree
+template <bool kAbs>
 __global__ void __launch_bounds__(kBlock) coldot_kernel(int r0, int r1, int t, const double* __restrict__ A, const double* __restrict__ B,
                                                         double* __restrict__ out) {
   __shared__ double sh[kBlock];
@@ -125,7 +127,7 @@ __global__ void __launch_bounds__(kBlock) coldot_kernel(int r0, int r1, int t, c
   const int per = (len + kBlock - 1) / kBlock;
   const int b = r0 + threadIdx.x * per, e = min(b + per, r1);
   double a = 0.;
-  for (int i = b; i < e; ++i) a += A[(size_t)i * t + c] * B[(size_t)i * t + c];
+  for (int i = b; i < e; ++i) a += kAbs ? fabs(A[(size_t)i * t + c]) : A[(size_t)i * t + c] * B[(size_t)i * t + c];
   sh[threadIdx.x] = a;
   __syncthreads();
   for (int o = kBlock / 2; o > 0; o >>= 1) {
@@ -187,9 +189,10 @@ int gm_grid(const gpbdev_grouped_multi* h, int64_t rows_or_len, int per) {
   return (int)std::max<int64_t>(1, std::min<int64_t>((rows_or_len * per + gmk::kBlock - 1) / gmk::kBlock, (int64_t)h->num_sms * 16));
 }
 
-// column dots over rows [r0, r1) -> out (host)
+// column dots over rows [r0, r1) -> out (host); B = nullptr: column sums of |A| (L1 norms)
 int gm_dots(gpbdev_grouped_multi* h, int r0, int r1, int t, const double* A, const double* B, double* out) {
-  gmk::coldot_kernel<<<t, gmk::kBlock, 0, h->stream>>>(r0, r1, t, A, B, h->dots);
+  if (B) gmk::coldot_kernel<false><<<t, gmk::kBlock, 0, h->stream>>>(r0, r1, t, A, B, h->dots);
+  else gmk::coldot_kernel<true><<<t, gmk::kBlock, 0, h->stream>>>(r0, r1, t, A, nullptr, h->dots);
   GCUDA(cudaGetLastError());
   h->launches += 1;
   GCUDA(cudaMemcpyAsync(h->dots_host, h->dots, sizeof(double) * t, cudaMemcpyDeviceToHost, h->stream));
@@ -256,9 +259,9 @@ int gm_pcg(gpbdev_grouped_multi* h, int t, const double* B, double* X, bool warm
   GCUDA(cudaMemcpyAsync(h->R, B, sizeof(double) * len, cudaMemcpyDeviceToDevice, h->stream));
   std::vector<double> rz(t), rz_new(t), hv(t), rr(t), a(t, 1.), a_old(t, 1.), b(t, 0.), b_old(t, 0.);
   if (!lanczos) {
-    double b2;  // the reference returns zero when |B|_1 < 1e-100 (THRESHOLD_ZERO_RHS_CG_); |B|^2 underflows to 0 there
-    if (gm_dots(h, 0, h->G, 1, B, B, &b2)) return -1;
-    if (b2 == 0.) {
+    double b1;  // the reference returns zero when |B|_1 < 1e-100 (THRESHOLD_ZERO_RHS_CG_)
+    if (gm_dots(h, 0, h->G, 1, B, nullptr, &b1)) return -1;
+    if (b1 < 1e-100) {
       GCUDA(cudaMemsetAsync(X, 0, sizeof(double) * len, h->stream));
       return 0;
     }

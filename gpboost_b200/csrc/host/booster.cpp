@@ -302,6 +302,8 @@ void Booster::Boosting() {
 
 bool Booster::TrainOneIter() {
   if (learner_ == nullptr) Fatal("This Booster was loaded from a model string / file and has no training data (prediction only)");
+  // refused before BoostFromAverage changes the scores, so that a refused iteration leaves the booster as it was
+  if (leaves_newton_update_) re_model_->CheckNewtonUpdateLeafValues(num_leaves_);
   double init_score = 0.;
   if (models_.empty() && boost_from_average_) {  // BoostFromAverage (gbdt.cpp:376-408): mean label for L2 (also with a Gaussian GP model)
     double suml = 0.;

@@ -1264,9 +1264,15 @@ void REModel::CalcGradientDevice(double* y_dev, bool response_is_current) {
   DevCheck(gpbdev_vecchia_yaux_device(engine_, y_dev, 1. / cov_pars_[0]));
 }
 
-void REModel::NewtonUpdateLeafValuesDevice(const int32_t* leaf_of_row_dev, int num_leaves, const double* grad_dev, double* leaf_values) {
+void REModel::CheckNewtonUpdateLeafValues(int num_leaves) const {
   if (!gauss_) Fatal("Newton updates for leaf values is only supported for Gaussian data");  // re_model_template.h:4986-4988
   if (engine_ == nullptr) Fatal("Newton updates for leaf values are only built for the Vecchia GP model in the CUDA engine");
+  if (num_leaves > 256)
+    Fatal("Newton updates for leaf values are built for at most 256 leaves in the CUDA engine (num_leaves = " + std::to_string(num_leaves) + ")");
+}
+
+void REModel::NewtonUpdateLeafValuesDevice(const int32_t* leaf_of_row_dev, int num_leaves, const double* grad_dev, double* leaf_values) {
+  CheckNewtonUpdateLeafValues(num_leaves);
   const int L = num_leaves;
   std::vector<double> M((size_t)L * L), rhs((size_t)L);
   DevCheck(gpbdev_vecchia_newton_system(engine_, leaf_of_row_dev, L, grad_dev, M.data(), rhs.data()));

@@ -71,6 +71,8 @@ class REModel {
   // REModel::NewtonUpdateLeafValues (re_model.cpp:1298-1310 -> re_model_template.h:4982-5063), device-resident: leaf ids and the
   // gradient of the tree that was just grown stay in HBM; only the L x L system comes to the host. After CalcGradient*.
   void NewtonUpdateLeafValuesDevice(const int32_t* leaf_of_row_dev, int num_leaves, const double* grad_dev, double* leaf_values);
+  // throws unless this model has the device Newton step for trees of up to num_leaves leaves (Gaussian Vecchia, at most 256)
+  void CheckNewtonUpdateLeafValues(int num_leaves) const;
   // GPB_SetPredictionData (c_api.h:1601-1613): prediction locations / neighbour count kept for later Predict calls
   // covariate_data_pred: num_data_pred x num_covariates column-major, required exactly when the model has covariates
   void SetPredictionData(int32_t num_data_pred, const double* gp_coords_data_pred, const double* covariate_data_pred,
