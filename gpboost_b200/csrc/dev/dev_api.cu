@@ -340,7 +340,7 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
       default: GPB_PICK2(gpb::COV_GAUSSIAN); break;
     }
 #undef GPB_PICK2
-    const size_t smem2 = sizeof(double) * gpb::kWarpsPerBlock * 2 * (gpb::kNll2Half + 64);
+    const size_t smem2 = sizeof(double) * gpb::kWarpsPerBlock * 2 * (gpb::kNll2Half + gpb::kNll2Pts);
     CUDA_TRY(cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
     CUDA_TRY(cudaFuncSetAttribute(k2, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     int per_sm2 = 0;

@@ -19,6 +19,7 @@
 namespace gpb {
 
 constexpr int kNll2Half = 32 * kLd + 2;  // doubles per half: 32 x 33 matrix + 2 pad -> halves 16 bytes apart modulo 128 bytes
+constexpr int kNll2Pts = 96;             // doubles per half: points 0..30 and a copy of points 0..15 behind them (47 x 2, padded)
 // ---- covariance evaluation of this kernel. ncu of the first version had 52 % of
 // the stall samples in the pair-covariance rounds: every round a serial chain of ~33 dependent FP64 instructions (the shared-memory
 // store of round r ordered the load of round r + 1 behind it), issued at the DFMA latency. Here
@@ -126,9 +127,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MODE == MODE_GRAD ? GPB_N
   extern __shared__ __align__(16) double smem_raw[];
   const int lane = threadIdx.x & 31, hl = lane & 15, hh = lane >> 4, wib = threadIdx.x >> 5;
   const int hbase = lane & 16;  // first lane of my half
-  // per-warp shared layout: two halves of [matrix 32 x kLd + 2 | points 32 x 2]
-  double* S = smem_raw + (size_t)wib * (2 * (kNll2Half + 64)) + (size_t)hh * kNll2Half;
-  double* pts = smem_raw + (size_t)wib * (2 * (kNll2Half + 64)) + 2 * kNll2Half + (size_t)hh * 64;
+  // per-warp shared layout: two matrices of 32 x kLd + 2, then two point buffers of kNll2Pts
+  double* S = smem_raw + (size_t)wib * (2 * (kNll2Half + kNll2Pts)) + (size_t)hh * kNll2Half;
+  double* pts = smem_raw + (size_t)wib * (2 * (kNll2Half + kNll2Pts)) + 2 * kNll2Half + (size_t)hh * kNll2Pts;
   const int64_t gwarp = (int64_t)blockIdx.x * kWarpsPerBlock + wib, nwarps = (int64_t)gridDim.x * kWarpsPerBlock;
   const int m = p.m;
   const double var = p.var;
@@ -172,18 +173,33 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MODE == MODE_GRAD ? GPB_N
   fetch_data();
   fetch_idx(row_of(it + nwarps), row_of(it + nwarps) < p.row_end, sn_lo, sn_hi);
 
+  // ---- pair covariances: round r -> offset t = r / 2 + 1, own point pi = hl + 16 (r & 1), partner o = (pi + t) mod P.
+  // Every address of a round is a per-lane base plus a compile-time offset (the lane-dependent addresses of the 30 rounds, kept
+  // across the pair loop, were what spilled): point s sits at pts2[s] and, for s < 16, again at pts2[s + P], so the partner is
+  // read at pts2[pi + t] without a wrap; pair (min, max) sits at S[min * kLd + max], i.e. at pi (kLd + 1) + t when pi + t < P and
+  // at pi (kLd + 1) + (t - P) kLd when the partner wraps (only hi rounds wrap: hl + t <= 30). The padded pair (lane 15, odd
+  // rounds, pi = 31) is computed on a copied point and not stored.
+  double2* pts2 = reinterpret_cast<double2*>(pts);
+  auto Sd = [&]() { return S + hl * (kLd + 1); };         // S[hl][hl]: base of the lo rounds
+  auto Sh = [&]() { return S + (hl + 16) * (kLd + 1); };  // S[hl + 16][hl + 16]: base of the hi rounds
+  const bool pad_lane = hl + 16 >= P;
+
   for (; __any_sync(0xffffffffu, active); ) {
     const int q = i < m ? (int)i : m;
     const bool real_lo = s_lo >= 0, real_hi = s_hi >= 0;
-    const double2 my_lo = make_double2(c_lo.x * sc, c_lo.y * sc), my_hi = make_double2(c_hi.x * sc, c_hi.y * sc);
     const double yl = y_lo, yh = y_hi;
-    if (real_lo) *reinterpret_cast<double2*>(pts + hl * 2) = my_lo;
-    if (real_hi) *reinterpret_cast<double2*>(pts + (hl + 16) * 2) = my_hi;
+    const double2 my_lo = make_double2(c_lo.x * sc, c_lo.y * sc), my_hi = make_double2(c_hi.x * sc, c_hi.y * sc);
+    if (real_lo) { pts2[hl] = my_lo; pts2[hl + P] = my_lo; }
+    if (real_hi) pts2[hl + 16] = my_hi;
     // which point slots of my half are real (bit s): slots 0..q-1 and slot MT
     const unsigned blo = __ballot_sync(0xffffffffu, real_lo), bhi = __ballot_sync(0xffffffffu, real_hi);
     const unsigned real_mask = ((blo >> hbase) & 0xffffu) | (((bhi >> hbase) & 0xffffu) << 16);
     // no dummy slots anywhere in the warp (supplied neighbour sets may pad rows i >= m with -1 too)
     const bool full = (__all_sync(0xffffffffu, real_mask == (1u << P) - 1u || !active)) != 0;
+    // bit t: the pair of round t (lo / hi) is kept; dummy slots are zeroed unless the whole warp is free of them
+    const unsigned long long real2 = (unsigned long long)real_mask | ((unsigned long long)real_mask << P);
+    const unsigned keep_lo = full ? ~0u : (real_lo ? real_mask >> hl : 0u);
+    const unsigned keep_hi = full ? ~0u : (real_hi ? (unsigned)(real2 >> (hl + 16)) : 0u);
     const bool was_active = active;
     // next pair
     const int64_t it_n = it + nwarps;
@@ -191,15 +207,11 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MODE == MODE_GRAD ? GPB_N
     const bool active_n = i_n < p.row_end;
     __syncwarp();
 
-    // ---- pair covariances: round r -> offset t = r / 2 + 1, own point pi = hl + 16 (r & 1)
     // The rounds run in groups of G: the G values stay in registers until the group's rounds are done, then they are stored — a
     // store between two point loads would order the second load behind it (same address space, run-time indices) and serialise the
     // rounds' dependent FP64 chains (the state of the first version of this kernel).
     constexpr int NR = 2 * (MT / 2);
-#ifndef GPB_NLL2_GROUP
-#define GPB_NLL2_GROUP 6
-#endif
-    constexpr int G = GRAD ? 6 : GPB_NLL2_GROUP;
+    constexpr int G = 6;
     static_assert(NR % G == 0, "group size must divide the number of rounds");
     double gp[(GRAD && !GP_SMEM) ? NR : 1];
 #pragma unroll
@@ -210,11 +222,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MODE == MODE_GRAD ? GPB_N
         const int r = r0 + j;
         const int t = (r >> 1) + 1;
         const bool odd = (r & 1) != 0;
-        const int pi = hl + (odd ? 16 : 0);
-        int o = pi + t;
-        if (o >= P) o -= P;
-        if (pi >= P) o = 0;
-        const double2 po = *reinterpret_cast<const double2*>(pts + o * 2);
+        const double2 po = pts2[hl + (odd ? 16 : 0) + t];
         const double2 me = odd ? my_hi : my_lo;
         const double dx = me.x - po.x, dy = me.y - po.y;
         const double d2s = fma(dy, dy, fma(dx, dx, 1e-300));
@@ -227,18 +235,19 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, MODE == MODE_GRAD ? GPB_N
         const int r = r0 + j;
         const int t = (r >> 1) + 1;
         const bool odd = (r & 1) != 0;
-        const int pi = hl + (odd ? 16 : 0);
-        const bool valid = pi < P;
-        int o = pi + t;
-        if (o >= P) o -= P;
-        if (!valid) o = 0;
-        // dummy slots: zero unless the whole warp is free of them; the one padded pair (lane 15, odd rounds) goes to the unused column 31
-        const bool keep = ((full ? 1u : 0u) | ((odd ? (unsigned)real_hi : (unsigned)real_lo) & (real_mask >> o) & 1u)) != 0u;  // no branches
+        const bool keep = (((odd ? keep_hi : keep_lo) >> t) & 1u) != 0u;  // no branches
         const double v = keep ? val[j] : 0.;
-        S[valid ? min(pi, o) * kLd + max(pi, o) : 31 * kLd + hl] = v;
-        if (GRAD) {  // derivative value: 0 for padded / dummy pairs; pair (a, b), a < b -> column b, row a (padded pair: column 31)
-          if (GP_SMEM) S[valid ? max(pi, o) * kLd + min(pi, o) : 31 * kLd + 16 + hl] = keep ? gval[j] : 0.;
-          else gp[r] = (keep && valid) ? gp[r] : 0.;
+        // derivative value: 0 for padded / dummy pairs; pair (a, b), a < b -> column b, row a
+        if (!odd) {
+          Sd()[t] = v;
+          if (GRAD) { if (GP_SMEM) Sd()[t * kLd] = keep ? gval[j] : 0.; else gp[r] = keep ? gp[r] : 0.; }
+        } else {
+          const bool wrap = hl + 16 + t >= P;
+          if (!pad_lane) {
+            if (wrap) Sh()[(t - P) * kLd] = v; else Sh()[t] = v;
+            if (GRAD && GP_SMEM) { if (wrap) Sh()[t - P] = keep ? gval[j] : 0.; else Sh()[t * kLd] = keep ? gval[j] : 0.; }
+          }
+          if (GRAD && !GP_SMEM) gp[r] = (keep && !pad_lane) ? gp[r] : 0.;
         }
       }
     }
