@@ -284,7 +284,7 @@ class GPModel(object):
         return buf.value.decode()
 
     def predict(self, y, gp_coords_pred, cov_pars, predict_var=False, predict_response=True, vecchia_pred_type=None,
-                num_neighbors_pred=-1, X_pred=None):
+                num_neighbors_pred=-1, X_pred=None, cluster_ids_pred=None):
         """Predictive mean (and variance) at new locations (GPModel.predict, basic.py:6168-6520 -> GPB_SetPredictionData,
         GPB_PredictREModel), GP part only. Returns dict(mu, var). This library does not export the prediction entries
         yet (SURVEY §8 f1); with `_lib` = the reference library this produces the golden vectors for them."""
@@ -303,18 +303,30 @@ class GPModel(object):
                 raise GPBoostError("Incorrect number of data points in X_pred")
             self._Xpred_c = np.ascontiguousarray(X_pred.flatten(order="F"))
             xp_c = _dptr(self._Xpred_c)
+        cl_c = self._cluster_ids_pred_ptr(cluster_ids_pred, npred)
         self._safe_call(self._LIB.GPB_SetPredictionData(
-            self.handle, ctypes.c_int32(npred), None, None, None, _dptr(Xp), None, xp_c,
+            self.handle, ctypes.c_int32(npred), cl_c, None, None, _dptr(Xp), None, xp_c,
             c_str(vecchia_pred_type) if vecchia_pred_type else None, ctypes.c_int(num_neighbors_pred), ctypes.c_double(-1.),
             ctypes.c_int(-1), ctypes.c_int(-1)))
         out = np.zeros(npred * (2 if predict_var else 1), dtype=np.float64)
         self._safe_call(self._LIB.GPB_PredictREModel(
             self.handle, y_c, ctypes.c_int32(npred), _dptr(out), ctypes.c_bool(False), ctypes.c_bool(predict_var),
             ctypes.c_bool(predict_response), ctypes.c_bool(False), ctypes.c_bool(False), ctypes.c_int(0), ctypes.c_int(0),
-            None, None, None, _dptr(Xp), None, cp_c, xp_c, ctypes.c_bool(True), None, None))
+            cl_c, None, None, _dptr(Xp), None, cp_c, xp_c, ctypes.c_bool(True), None, None))
         return {"mu": out[:npred].copy(), "var": out[npred:].copy() if predict_var else None}
 
-    def set_prediction_data(self, gp_coords_pred=None, vecchia_pred_type=None, num_neighbors_pred=None, X_pred=None):
+    def _cluster_ids_pred_ptr(self, cluster_ids_pred, npred):
+        """int32 labels of the independent realizations at the prediction points (basic.py: cluster_ids_pred); a label without training
+        data predicts from the prior"""
+        if cluster_ids_pred is None:
+            return None
+        self._cluster_ids_pred_c = np.ascontiguousarray(np.asarray(cluster_ids_pred).reshape(-1).astype(np.int32))
+        if len(self._cluster_ids_pred_c) != npred:
+            raise ValueError("Incorrect number of data points in 'cluster_ids_pred'")
+        return self._cluster_ids_pred_c.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+
+    def set_prediction_data(self, gp_coords_pred=None, vecchia_pred_type=None, num_neighbors_pred=None, X_pred=None,
+                            cluster_ids_pred=None):
         """Set the prediction data (GPModel.set_prediction_data, basic.py): the GP coordinates of the validation data the GPBoost
         algorithm predicts at with `use_gp_model_for_validation=True`."""
         if gp_coords_pred is None and X_pred is None and vecchia_pred_type is None and num_neighbors_pred is None:
@@ -339,8 +351,11 @@ class GPModel(object):
             npred = X_pred.shape[0]
             self._Xpred_saved_c = np.ascontiguousarray(X_pred.flatten(order="F"))
             xp_c = _dptr(self._Xpred_saved_c)
+        cl_c = self._cluster_ids_pred_ptr(cluster_ids_pred, npred) if cluster_ids_pred is not None and npred else None
+        if cluster_ids_pred is not None and not npred:
+            raise ValueError("'cluster_ids_pred' needs 'gp_coords_pred'")
         self._safe_call(self._LIB.GPB_SetPredictionData(
-            self.handle, ctypes.c_int32(npred), None, None, None, coords_c, None, xp_c,
+            self.handle, ctypes.c_int32(npred), cl_c, None, None, coords_c, None, xp_c,
             c_str(vecchia_pred_type) if vecchia_pred_type else None,
             ctypes.c_int(-1 if num_neighbors_pred is None else int(num_neighbors_pred)), ctypes.c_double(-1.),
             ctypes.c_int(-1), ctypes.c_int(-1)))

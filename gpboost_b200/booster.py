@@ -221,7 +221,7 @@ class Booster(object):
 
     def predict(self, data, start_iteration=0, num_iteration=None, raw_score=None, pred_leaf=False, pred_latent=False, gp_coords_pred=None,
                 predict_var=False, cov_pars=None, ignore_gp_model=False, offset_pred=None, num_neighbors_pred=-1, pred_contrib=False,
-                predict_cov_mat=False, sample_posterior=False):
+                predict_cov_mat=False, sample_posterior=False, cluster_ids_pred=None):
         """Prediction at new data (Booster.predict, basic.py:3376-3802). Without a `gp_model` (or with `ignore_gp_model=True`): the
         tree ensemble's scores, or with `pred_leaf=True` the (nrow, trees) leaf indices. With a Gaussian `gp_model`: the reference's
         dict — `pred_latent=True`: fixed_effect, random_effect_mean, random_effect_cov (the variances, with `predict_var`);
@@ -252,7 +252,8 @@ class Booster(object):
         fixed_effect_train = self._predict_for_mat(self.train_set.data, C_API_PREDICT_RAW_SCORE, start_iteration, num_iteration)
         residual = self.train_set.label - fixed_effect_train
         re_pred = self.gp_model.predict(y=residual, gp_coords_pred=gp_coords_pred, cov_pars=cov_pars, predict_var=predict_var,
-                                        predict_response=not pred_latent, num_neighbors_pred=num_neighbors_pred)
+                                        predict_response=not pred_latent, num_neighbors_pred=num_neighbors_pred,
+                                        cluster_ids_pred=cluster_ids_pred)
         fixed_effect = self._predict_for_mat(data, C_API_PREDICT_RAW_SCORE, start_iteration, num_iteration)
         if len(fixed_effect) != len(re_pred["mu"]):
             raise GPBoostError("Number of data points in fixed effect (tree ensemble) and random effect are not equal")

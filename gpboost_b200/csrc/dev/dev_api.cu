@@ -86,6 +86,11 @@ __global__ void bt_apply_kernel(const double* __restrict__ A, const double* __re
   }
 }
 
+// dst[order[k]] = src[k]: results of a clustered prediction set (computed cluster by cluster) back to the caller's point order
+__global__ void scatter_order_kernel(const double* __restrict__ src, const int32_t* __restrict__ order, double* __restrict__ dst, int64_t n) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) dst[order[k]] = src[k];
+}
+
 __global__ void fill_kernel(double* p, int64_t n, double v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
 }
@@ -205,6 +210,9 @@ struct gpbdev_vecchia {
   double stored_var = 0., stored_range = 0., last_var = 0., last_range = 0.;
   int knn_replayed = 0;  // queries whose neighbour set was re-derived by the exact replay of the reference walk
   std::vector<int32_t> nn_host;  // kept for the lazy CSC build
+  // independent realizations (gpbdev_vecchia_create_clusters): cluster c holds the ordered rows [clu_start[c], clu_start[c + 1]);
+  // empty for an engine of one realization
+  std::vector<int64_t> clu_start;
   // linear regression covariates (covariates.cuh), lazy
   int p = 0;                       // number of covariates
   double* X = nullptr;             // n x p ROW-major, Vecchia order
@@ -393,8 +401,15 @@ int gpbdev_device_count(void) {
 namespace {
 
 int vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered, const int32_t* perm,
-                   const int32_t* nn, int64_t row_begin, int64_t row_end, bool search) {
+                   const int32_t* nn, int64_t row_begin, int64_t row_end, bool search, int num_clusters = 0,
+                   const int64_t* cluster_start = nullptr) {
   if (!out || !coords_ordered || !perm) return fail("gpbdev_vecchia_create: null argument");
+  if (num_clusters > 0) {
+    if (!cluster_start || cluster_start[0] != 0 || cluster_start[num_clusters] != n)
+      return fail("gpbdev_vecchia_create_clusters: cluster_start must run from 0 to n");
+    for (int c = 0; c < num_clusters; ++c)
+      if (cluster_start[c + 1] <= cluster_start[c]) return fail("gpbdev_vecchia_create_clusters: every cluster needs at least one row");
+  }
   if (n <= 0 || d <= 0 || d > 16) return fail("gpbdev_vecchia_create: need n > 0 and 1 <= dim <= 16");
   if (m < 1 || m > gpb::kBigMaxNeighbors)
     return fail("gpbdev_vecchia_create: num_neighbors must be in [1, " + std::to_string(gpb::kBigMaxNeighbors) +
@@ -451,6 +466,15 @@ int vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, c
   } else if (!search) {
     CUDA_TRY(cudaMemset(h->nn, 0xff, sizeof(int32_t) * n * m));
     h->nn_searched = false;
+  } else if (num_clusters > 0) {
+    h->clu_start.assign(cluster_start, cluster_start + num_clusters + 1);
+    std::string err;
+    gpb::KnnInfo info;
+    const int nl = gpb::knn_cluster_search(h->coords, coords_ordered, n, n, d, m, m, num_clusters, cluster_start, nullptr, h->nn, h->stream,
+                                           h->num_sms, &info, &err);
+    if (nl < 0) { gpbdev_vecchia_free(h); return fail("gpbdev_vecchia_create_clusters: device neighbour search failed: " + err); }
+    h->launches += nl;
+    h->knn_replayed = (int)info.replayed;
   } else {
     std::string err;
     gpb::KnnInfo info;
@@ -471,6 +495,12 @@ extern "C" {
 int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
                           const int32_t* perm, const int32_t* nn, int64_t row_begin, int64_t row_end) {
   return vecchia_create(out, device, n, d, m, coords_ordered, perm, nn, row_begin, row_end, true);
+}
+
+int gpbdev_vecchia_create_clusters(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
+                                   const int32_t* perm, int num_clusters, const int64_t* cluster_start) {
+  if (num_clusters < 1) return fail("gpbdev_vecchia_create_clusters: num_clusters must be positive");
+  return vecchia_create(out, device, n, d, m, coords_ordered, perm, nullptr, 0, n, true, num_clusters, cluster_start);
 }
 
 int gpbdev_vecchia_create_unsearched(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
@@ -502,6 +532,14 @@ int gpbdev_vecchia_get_nn(gpbdev_vecchia_t h, int32_t* nn_host) {
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   CUDA_TRY(cudaMemcpy(nn_host, h->nn, sizeof(int32_t) * h->n * h->m, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int gpbdev_vecchia_get_perm(gpbdev_vecchia_t h, int32_t* perm_host) {
+  if (!h || !perm_host) return fail("gpbdev_vecchia_get_perm: null argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  CUDA_TRY(cudaMemcpy(perm_host, h->perm, sizeof(int32_t) * h->n, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -617,6 +655,11 @@ struct gpbdev_vecchia_predset {
   int32_t* nn = nullptr;      // np x mp, indices into the observed points (Vecchia order)
   double* mean = nullptr;     // np: A_p y_N(p) of the last evaluation
   double* dvar = nullptr;     // np: D_p (transformed scale) of the last evaluation
+  // clustered set: the points are searched and evaluated cluster by cluster; order[k] = caller's index of point k, and the kernel
+  // writes mean_k / dvar_k before they are scattered to mean / dvar
+  int32_t* order = nullptr;
+  double* mean_k = nullptr;
+  double* dvar_k = nullptr;
 };
 
 extern "C" {
@@ -627,6 +670,7 @@ int gpbdev_vecchia_predset_create(gpbdev_vecchia_t h, const double* coords_pred_
   *out = nullptr;
   if (np <= 0) return fail("gpbdev_vecchia_predict: no prediction points");
   if (h->row_begin != 0 || h->row_end != h->n) return fail("gpbdev_vecchia_predict: prediction needs the whole model on this device (row-sharded engine)");
+  if (!h->clu_start.empty()) return fail("gpbdev_vecchia_predict: an engine of several clusters predicts through gpbdev_vecchia_predset_create_clusters");
   const int64_t n = h->n;
   const int d = h->d;
   int mp = (int)std::min<int64_t>(num_neighbors_pred, n);  // Vecchia_utils.cpp:752-755
@@ -666,6 +710,77 @@ int gpbdev_vecchia_predset_create(gpbdev_vecchia_t h, const double* coords_pred_
   return 0;
 }
 
+int gpbdev_vecchia_predset_create_clusters(gpbdev_vecchia_t h, const double* coords_pred_host, int64_t np, int num_neighbors_pred,
+                                           const int32_t* cluster_of_pred, gpbdev_vecchia_predset_t* out) {
+  if (!h || !coords_pred_host || !cluster_of_pred || !out) return fail("gpbdev_vecchia_predict: null argument");
+  *out = nullptr;
+  if (np <= 0) return fail("gpbdev_vecchia_predict: no prediction points");
+  if (h->row_begin != 0 || h->row_end != h->n) return fail("gpbdev_vecchia_predict: prediction needs the whole model on this device (row-sharded engine)");
+  const int64_t n = h->n;
+  const int d = h->d;
+  const std::vector<int64_t> obs_start = h->clu_start.empty() ? std::vector<int64_t>{0, n} : h->clu_start;
+  const int K = (int)obs_start.size() - 1;
+  int64_t max_obs = 0;
+  for (int c = 0; c < K; ++c) max_obs = std::max(max_obs, obs_start[c + 1] - obs_start[c]);
+  const int mp = (int)std::min<int64_t>(num_neighbors_pred, max_obs);  // Vecchia_utils.cpp:752-755, per cluster in the search
+  if (mp < 1 || mp > gpb::kBigMaxNeighbors)
+    return fail("gpbdev_vecchia_predict: num_neighbors_pred must be in [1, " + std::to_string(gpb::kBigMaxNeighbors) + "] for the CUDA Vecchia engine");
+  if ((n + np) >= (int64_t)2147483647 || np * (int64_t)mp >= (int64_t)2147483647) return fail("gpbdev_vecchia_predict: too many points for int32 indices");
+  // points grouped by cluster (cluster order, each cluster's points in the caller's order), points of no cluster (-1) last
+  std::vector<int64_t> cnt((size_t)K + 2, 0);
+  for (int64_t p = 0; p < np; ++p) {
+    const int32_t c = cluster_of_pred[p];
+    if (c < -1 || c >= K) return fail("gpbdev_vecchia_predict: cluster index " + std::to_string(c) + " of prediction point " + std::to_string(p) + " outside [-1, " + std::to_string(K) + ")");
+    ++cnt[(size_t)(c < 0 ? K : c) + 1];
+  }
+  for (int c = 0; c <= K; ++c) cnt[(size_t)c + 1] += cnt[(size_t)c];
+  std::vector<int64_t> pred_start((size_t)K + 1);
+  for (int c = 0; c <= K; ++c) pred_start[(size_t)c] = n + cnt[(size_t)c];
+  std::vector<int32_t> order((size_t)np);
+  {
+    std::vector<int64_t> fill(cnt.begin(), cnt.end() - 1);
+    for (int64_t p = 0; p < np; ++p) {
+      const int32_t c = cluster_of_pred[p];
+      order[(size_t)fill[(size_t)(c < 0 ? K : c)]++] = (int32_t)p;
+    }
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  const int64_t na = n + np;
+  std::vector<double> call((size_t)na * d);
+  CUDA_TRY(cudaMemcpy(call.data(), h->coords, sizeof(double) * n * d, cudaMemcpyDeviceToHost));
+  for (int64_t k = 0; k < np; ++k)
+    std::memcpy(call.data() + (size_t)(n + k) * d, coords_pred_host + (size_t)order[(size_t)k] * d, sizeof(double) * d);
+  auto* ps = new gpbdev_vecchia_predset();
+  ps->h = h; ps->np = np; ps->mp = mp;
+  double* call_dev = nullptr;
+  auto release = [&]() { cudaFree(call_dev); gpbdev_vecchia_predset_free(ps); };
+  cudaError_t e = cudaMalloc(&call_dev, sizeof(double) * na * d);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->nn, sizeof(int32_t) * np * mp);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->qcoords, sizeof(double) * np * d);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->mean, sizeof(double) * np);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->dvar, sizeof(double) * np);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->mean_k, sizeof(double) * np);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->dvar_k, sizeof(double) * np);
+  if (e == cudaSuccess) e = cudaMalloc(&ps->order, sizeof(int32_t) * np);
+  if (e == cudaSuccess) e = cudaMemcpy(ps->order, order.data(), sizeof(int32_t) * np, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(call_dev, call.data(), sizeof(double) * na * d, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) { release(); return fail(std::string("gpbdev_vecchia_predict: ") + cudaGetErrorString(e)); }
+  std::string err;
+  gpb::KnnInfo info;
+  const int nl = gpb::knn_cluster_search(call_dev, call.data(), na, n, d, mp, num_neighbors_pred, K, obs_start.data(), pred_start.data(),
+                                         ps->nn, h->stream, h->num_sms, &info, &err);
+  if (nl < 0) { release(); return fail("gpbdev_vecchia_predict: device neighbour search failed: " + err); }
+  h->launches += nl;
+  e = cudaMemcpyAsync(ps->qcoords, call_dev + (size_t)n * d, sizeof(double) * np * d, cudaMemcpyDeviceToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  cudaFree(call_dev);
+  call_dev = nullptr;
+  if (e != cudaSuccess) { release(); return fail(std::string("gpbdev_vecchia_predict: ") + cudaGetErrorString(e)); }
+  *out = ps;
+  return 0;
+}
+
 int gpbdev_vecchia_predset_eval(gpbdev_vecchia_predset_t ps, int cov_type, double var, double range, const double** mean_dev,
                                 const double** var_dev) {
   if (!ps || !ps->h) return fail("gpbdev_vecchia_predset_eval: null argument");
@@ -676,7 +791,8 @@ int gpbdev_vecchia_predset_eval(gpbdev_vecchia_predset_t ps, int cov_type, doubl
   CUDA_TRY(cudaSetDevice(h->device));
   gpb::BigArgs b;
   b.coords = h->coords; b.y = h->y; b.nn = ps->nn; b.qcoords = ps->qcoords;
-  b.A = nullptr; b.Dinv = nullptr; b.w = nullptr; b.pred_mean = ps->mean; b.pred_var = ps->dvar; b.partials = nullptr;
+  b.A = nullptr; b.Dinv = nullptr; b.w = nullptr; b.partials = nullptr;
+  b.pred_mean = ps->order ? ps->mean_k : ps->mean; b.pred_var = ps->order ? ps->dvar_k : ps->dvar;
   b.row_begin = 0; b.row_end = ps->np; b.m = ps->mp; b.d = d;
   b.var = var; b.range = range; b.diag_nb = var + 1.; b.diag_obs = var;  // Vecchia_utils.cpp:1940-1952 (nugget on the neighbour block), :1925-1931
   BigKernel bk = pick_big_kernel(cov_type, gpb::BIG_PRED);
@@ -686,6 +802,13 @@ int gpbdev_vecchia_predset_eval(gpbdev_vecchia_predset_t ps, int cov_type, doubl
   bk<<<grid, 128, bsmem, h->stream>>>(b);
   CUDA_TRY(cudaGetLastError());
   h->launches += 1;
+  if (ps->order) {  // rows of a point without observed neighbours are all -1: mean 0 and D_p = var, the prior
+    const int sg = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)h->num_sms * 4, (ps->np + 255) / 256));
+    scatter_order_kernel<<<sg, 256, 0, h->stream>>>(ps->mean_k, ps->order, ps->mean, ps->np);
+    scatter_order_kernel<<<sg, 256, 0, h->stream>>>(ps->dvar_k, ps->order, ps->dvar, ps->np);
+    CUDA_TRY(cudaGetLastError());
+    h->launches += 2;
+  }
   CUDA_TRY(cudaStreamSynchronize(h->stream));  // the results are read on other streams (the booster's metric kernel) or copied out
   if (mean_dev) *mean_dev = ps->mean;
   if (var_dev) *var_dev = ps->dvar;
@@ -696,18 +819,26 @@ int gpbdev_vecchia_predset_free(gpbdev_vecchia_predset_t ps) {
   if (!ps) return 0;
   if (ps->h) cudaSetDevice(ps->h->device);
   cudaFree(ps->qcoords); cudaFree(ps->nn); cudaFree(ps->mean); cudaFree(ps->dvar);
+  cudaFree(ps->order); cudaFree(ps->mean_k); cudaFree(ps->dvar_k);
   delete ps;
   return 0;
 }
 
 int gpbdev_vecchia_predict(gpbdev_vecchia_t h, int cov_type, double var, double range, const double* coords_pred_host, int64_t np,
                            int num_neighbors_pred, double* mean_out_host, double* var_out_host) {
+  return gpbdev_vecchia_predict_clusters(h, cov_type, var, range, coords_pred_host, np, num_neighbors_pred, nullptr, mean_out_host,
+                                         var_out_host);
+}
+
+int gpbdev_vecchia_predict_clusters(gpbdev_vecchia_t h, int cov_type, double var, double range, const double* coords_pred_host, int64_t np,
+                                    int num_neighbors_pred, const int32_t* cluster_of_pred, double* mean_out_host, double* var_out_host) {
   if (!h || !coords_pred_host || !mean_out_host || !var_out_host) return fail("gpbdev_vecchia_predict: null argument");
   if (np <= 0) return fail("gpbdev_vecchia_predict: no prediction points");
   if (cov_type < 0 || cov_type > 3) return fail("gpbdev_vecchia_predict: unknown covariance id");
   if (!(var > 0.) || !(range > 0.)) return fail("gpbdev_vecchia_predict: covariance parameters must be positive");
   gpbdev_vecchia_predset_t ps = nullptr;
-  if (gpbdev_vecchia_predset_create(h, coords_pred_host, np, num_neighbors_pred, &ps)) return -1;
+  if (cluster_of_pred ? gpbdev_vecchia_predset_create_clusters(h, coords_pred_host, np, num_neighbors_pred, cluster_of_pred, &ps)
+                      : gpbdev_vecchia_predset_create(h, coords_pred_host, np, num_neighbors_pred, &ps)) return -1;
   const double *mean_dev = nullptr, *var_dev = nullptr;
   if (gpbdev_vecchia_predset_eval(ps, cov_type, var, range, &mean_dev, &var_dev)) { gpbdev_vecchia_predset_free(ps); return -1; }
   cudaError_t e = cudaMemcpy(mean_out_host, mean_dev, sizeof(double) * np, cudaMemcpyDeviceToHost);
@@ -810,6 +941,7 @@ int gpbdev_vecchia_set_coord_scale(gpbdev_vecchia_t h, const double* scale) {
 int gpbdev_vecchia_search_neighbors(gpbdev_vecchia_t h) {
   if (!h) return fail("gpbdev_vecchia_search_neighbors: null handle");
   if (h->row_begin != 0 || h->row_end != h->n) return fail("gpbdev_vecchia_search_neighbors: needs the whole model on this device");
+  if (!h->clu_start.empty()) return fail("gpbdev_vecchia_search_neighbors: not supported for an engine of several clusters");
   CUDA_TRY(cudaSetDevice(h->device));
   std::vector<double> ch((size_t)h->n * h->d);  // the search replays ties on the host copy of the same coordinates
   CUDA_TRY(cudaMemcpyAsync(ch.data(), h->coords, sizeof(double) * h->n * h->d, cudaMemcpyDeviceToHost, h->stream));

@@ -48,6 +48,20 @@ struct KnnInfo {
   int g[3] = {0, 0, 0};
 };
 
+// Independent realizations (cluster_ids): the reference searches every cluster on its own (one find_nearest_neighbors_Vecchia_fast
+// call per cluster, Vecchia_utils.cpp:1129-1184, prediction :1784-1800). Here the clusters are consecutive id ranges of one
+// search: cluster c's candidates are the ids [cand_lo, cand_lo + ncand) (its observed points), its points (candidates, and for
+// prediction its prediction points behind them) hold the positions [seg_lo, seg_end) of the sorted coordinate sums, sorted within
+// the cluster only, so rank differences, the walk and its pruning see the cluster alone. A query keeps m neighbours, the
+// reference's per-cluster cap of num_neighbors (:752-755); its nn row is -1 padded to the search's width. Clusters with more than
+// 4096 candidates (d <= 3) get their own cell grid (cells [cell_off, cell_off + g0 g1 g2)); their queries at local index
+// brute_end and above use it.
+struct KnnClu {
+  int64_t cand_lo, ncand, seg_lo, seg_end, cell_off, brute_end;
+  int m, grid;
+  KnnGrid gr;
+};
+
 __device__ __forceinline__ double knn_sqdist(const double* __restrict__ a, const double* __restrict__ b, int d) {
   double s = 0.;
   for (int k = 0; k < d; ++k) {
@@ -141,16 +155,17 @@ __device__ __forceinline__ void knn_offer(KnnTop<KS>& t, bool valid, double s, i
 // floating point it can when the comparison is decided by rounding (equidistant points on lattices). If every
 // neighbour found here satisfies smd <= d * T_final the reference provably visited all of them and the results are
 // identical; otherwise the query is queued for knn_walk_kernel, which replays the reference's walk exactly.
+// keep: neighbours kept (the list's first keep entries), width: length of the nn row (keep < width: -1 behind them)
 template <int KS>
-__device__ __forceinline__ void knn_finish(int64_t i, int lane, int m, int d, const KnnTop<KS>& t, const double* __restrict__ csum,
+__device__ __forceinline__ void knn_finish(int64_t i, int lane, int keep, int width, int d, const KnnTop<KS>& t, const double* __restrict__ csum,
                                            int32_t* __restrict__ nn_row, int32_t* __restrict__ flagged, int* __restrict__ nflag) {
-  const double tfin = t.s_at(m - 1);
+  const double tfin = t.s_at(keep - 1);
   bool risky = false;
 #pragma unroll
   for (int k = 0; k < KS; ++k) {
     const int p = k * 32 + lane;
-    if (p < m) {
-      nn_row[p] = t.id[k];
+    if (p < width) nn_row[p] = p < keep ? t.id[k] : -1;
+    if (p < keep) {
       if (t.id[k] >= 0) {
         const double dd = __dsub_rn(csum[t.id[k]], csum[i]);
         const double smd = __dmul_rn(dd, dd);
@@ -167,27 +182,37 @@ __device__ __forceinline__ void knn_finish(int64_t i, int lane, int m, int d, co
 // strict-'<' replacement and stable insertion (utils.h:250-262).
 // Candidates of query i are the points c < i with c <= end_search_at (training: end_search_at = n - 1; prediction points are
 // appended behind the observed ones and search the observed ones only, Vecchia_utils.cpp:1784-1800). nn row of query i = i - row0.
-template <int KS>
+// CLU: clusters (KnnClu): query i walks its cluster's segment of the sums, candidates are its cluster's ids below its local index
+template <int KS, bool CLU = false>
 __global__ void knn_walk_kernel(const double* __restrict__ coords, const double* __restrict__ csum,
-                                const int32_t* __restrict__ sort_sum, const int32_t* __restrict__ pos, int64_t n, int d, int m,
+                                const int32_t* __restrict__ sort_sum, const int32_t* __restrict__ pos, int64_t n, int d, int width,
                                 int64_t end_search_at, int64_t row0,
-                                const int32_t* __restrict__ flagged, const int* __restrict__ nflag, int32_t* __restrict__ nn) {
+                                const int32_t* __restrict__ flagged, const int* __restrict__ nflag, int32_t* __restrict__ nn,
+                                const KnnClu* __restrict__ clus = nullptr, const int32_t* __restrict__ clu_of = nullptr,
+                                const int32_t* __restrict__ loc_of = nullptr) {
   const int nf = *nflag;
   for (int f = blockIdx.x * blockDim.x + threadIdx.x; f < nf; f += gridDim.x * blockDim.x) {
     const int64_t i = flagged[f];
+    int m = width;
+    int64_t seg_lo = 0, seg_last = n - 1, cand_lo = 0, cand_end = min(i, end_search_at + 1);
+    if (CLU) {
+      const KnnClu& C = clus[clu_of[i]];
+      m = C.m; seg_lo = C.seg_lo; seg_last = C.seg_end - 1;
+      cand_lo = C.cand_lo; cand_end = C.cand_lo + min((int64_t)loc_of[i], C.ncand);
+    }
     double sq[32 * KS];
     int id[32 * KS];
     for (int j = 0; j < m; ++j) { sq[j] = INFINITY; id[j] = -1; }
     bool down = true, up = true;
     int64_t up_i = pos[i], down_i = pos[i];
     while (up || down) {
-      if (down_i == 0) down = false;
-      if (up_i == n - 1) up = false;
+      if (down_i == seg_lo) down = false;
+      if (up_i == seg_last) up = false;
       for (int dir = 0; dir < 2; ++dir) {
         if (dir == 0 ? !down : !up) continue;
         const int64_t p = dir == 0 ? --down_i : ++up_i;
         const int c = sort_sum[p];
-        if (c < i && c <= end_search_at) {
+        if (c >= cand_lo && c < cand_end) {
           const double dd = __dsub_rn(csum[c], csum[i]);
           const double smd = __dmul_rn(dd, dd);
           if (smd > __dmul_rn((double)d, sq[m - 1])) {
@@ -208,19 +233,33 @@ __global__ void knn_walk_kernel(const double* __restrict__ coords, const double*
         }
       }
     }
-    for (int j = 0; j < m; ++j) nn[(i - row0) * m + j] = id[j];
+    for (int j = 0; j < width; ++j) nn[(i - row0) * width + j] = j < m ? id[j] : -1;
   }
 }
 
+// clus != nullptr: every candidate of a cluster with a grid gets a cell of that grid (offset by its cell_off); every other point gets
+// the sentinel cell `sentinel` and sorts behind all cells
 __global__ void knn_cell_id_kernel(const double* __restrict__ coords, int64_t n, KnnGrid gr, uint32_t* __restrict__ cell,
-                                   int32_t* __restrict__ idx) {
+                                   int32_t* __restrict__ idx, const KnnClu* __restrict__ clus = nullptr,
+                                   const int32_t* __restrict__ clu_of = nullptr, uint32_t sentinel = 0) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     uint32_t c = 0;
+    if (clus != nullptr) {
+      const int cl = clu_of[i];
+      const KnnClu* C = cl >= 0 ? clus + cl : nullptr;
+      if (C == nullptr || C->grid < 0 || i < C->cand_lo || i >= C->cand_lo + C->ncand) {
+        cell[i] = sentinel;
+        idx[i] = (int32_t)i;
+        continue;
+      }
+      gr = C->gr;
+    }
     for (int k = gr.dim - 1; k >= 0; --k) {
       int ck = (int)floor((coords[i * gr.dim + k] - gr.lo[k]) * gr.inv_h[k]);
       ck = min(max(ck, 0), gr.g[k] - 1);
       c = c * (uint32_t)gr.g[k] + (uint32_t)ck;
     }
+    if (clus != nullptr) c += (uint32_t)clus[clu_of[i]].cell_off;
     cell[i] = c;
     idx[i] = (int32_t)i;
   }
@@ -236,51 +275,81 @@ __global__ void knn_cell_start_kernel(const uint32_t* __restrict__ sorted_cell, 
   }
 }
 
-// queries i in [q_begin, q_end): brute force over all j < min(i, end_search_at + 1) — warp per query
-template <int KS>
+// queries i in [q_begin, q_end): brute force over all j < min(i, end_search_at + 1) — warp per query.
+// CLU: over the ids [cand_lo, cand_lo + min(local index, ncand)) of the query's cluster, with the query's local index in place of i
+// (a query without a cluster gets an empty row; queries of a cluster's grid are left to knn_grid_kernel)
+template <int KS, bool CLU = false>
 __global__ void knn_brute_kernel(const double* __restrict__ coords, const int32_t* __restrict__ pos,
-                                 const double* __restrict__ csum, int d, int m, int64_t q_begin, int64_t q_end, int64_t end_search_at,
-                                 int64_t row0, int32_t* __restrict__ nn, int32_t* __restrict__ flagged, int* __restrict__ nflag) {
+                                 const double* __restrict__ csum, int d, int width, int64_t q_begin, int64_t q_end, int64_t end_search_at,
+                                 int64_t row0, int32_t* __restrict__ nn, int32_t* __restrict__ flagged, int* __restrict__ nflag,
+                                 const KnnClu* __restrict__ clus = nullptr, const int32_t* __restrict__ clu_of = nullptr,
+                                 const int32_t* __restrict__ loc_of = nullptr) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t i = q_begin + warp; i < q_end; i += nwarps) {
-    const int64_t ncand = min(i, end_search_at + 1);
-    int32_t* row = nn + (i - row0) * m;
+    int32_t* row = nn + (i - row0) * width;
+    int m = width;
+    int64_t li = i, lo = 0, ncand = min(i, end_search_at + 1);
+    if (CLU) {
+      const int cl = clu_of[i];
+      if (cl < 0) {
+        for (int p = lane; p < width; p += 32) row[p] = -1;
+        continue;
+      }
+      const KnnClu& C = clus[cl];
+      li = loc_of[i];
+      if (C.grid >= 0 && li >= C.brute_end) continue;
+      m = C.m; lo = C.cand_lo; ncand = min(li, C.ncand);
+    }
     // Vecchia_utils.cpp:788-813: rows i <= m take all predecessors, in index order. Later rows go through the walk even when
     // they have exactly m candidates (prediction with m = the number of observed points): distance order.
-    if (i <= m) {
-      for (int p = lane; p < m; p += 32) row[p] = p < ncand ? p : -1;
+    if (li <= m) {
+      for (int p = lane; p < width; p += 32) row[p] = p < ncand ? (int32_t)(lo + p) : -1;
       continue;
     }
     KnnTop<KS> top; top.init();
     const int pi = pos[i];
     for (int64_t j0 = 0; j0 < ncand; j0 += 32) {
-      const int64_t j = j0 + lane;
-      const bool valid = j < ncand;
+      const int64_t j = lo + j0 + lane;
+      const bool valid = j0 + lane < ncand;
       double s = 0.; int r = 0;
       if (valid) { s = knn_sqdist(coords + j * d, coords + i * d, d); r = knn_rank(pos[j], pi); }
       knn_offer<KS>(top, valid, s, r, (int)j, lane, m);
     }
-    knn_finish<KS>(i, lane, m, d, top, csum, row, flagged, nflag);
+    knn_finish<KS>(i, lane, m, width, d, top, csum, row, flagged, nflag);
   }
 }
 
 // queries i in [q_begin, n): cell-list search — warp per query, DIM in {1,2,3}
-template <int KS>
+// CLU: the query's cluster's grid (queries below its brute_end, and clusters without a grid, are left to knn_brute_kernel); a
+// cluster's cells hold its candidates only, so the valid part of a cell is still a prefix
+template <int KS, bool CLU = false>
 __global__ void knn_grid_kernel(const double* __restrict__ coords, const int32_t* __restrict__ pos,
                                 const double* __restrict__ csum, const int32_t* __restrict__ cell_start,
-                                const int32_t* __restrict__ sorted_idx, KnnGrid gr, int m, int64_t q_begin, int64_t n,
+                                const int32_t* __restrict__ sorted_idx, KnnGrid gr, int width, int64_t q_begin, int64_t n,
                                 int64_t end_search_at, int64_t row0,
-                                int32_t* __restrict__ nn, int32_t* __restrict__ flagged, int* __restrict__ nflag) {
+                                int32_t* __restrict__ nn, int32_t* __restrict__ flagged, int* __restrict__ nflag,
+                                const KnnClu* __restrict__ clus = nullptr, const int32_t* __restrict__ clu_of = nullptr,
+                                const int32_t* __restrict__ loc_of = nullptr) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int d = gr.dim;
   for (int64_t i = q_begin + warp; i < n; i += nwarps) {
+    int m = width;
+    int64_t id_end = min(i, end_search_at + 1);  // candidates: ids below this
+    const int32_t* cstart = cell_start;
+    if (CLU) {
+      const int cl = clu_of[i];
+      if (cl < 0) continue;
+      const KnnClu& C = clus[cl];
+      const int64_t li = loc_of[i];
+      if (C.grid < 0 || li < C.brute_end) continue;
+      m = C.m; id_end = C.cand_lo + min(li, C.ncand); gr = C.gr; cstart = cell_start + C.cell_off;
+    }
     KnnTop<KS> top; top.init();
     const int pi = pos[i];
-    const int64_t id_end = min(i, end_search_at + 1);  // candidates: ids below this
     int qc[3] = {0, 0, 0};
     for (int k = 0; k < d; ++k) {
       int ck = (int)floor((coords[i * d + k] - gr.lo[k]) * gr.inv_h[k]);
@@ -313,8 +382,8 @@ __global__ void knn_grid_kernel(const double* __restrict__ coords, const int32_t
           const int cx = qc[0] + dx, cy = qc[1] + dy, cz = qc[2] + dz;
           if (shell && cx >= 0 && cx < gr.g[0] && cy >= 0 && cy < gr.g[1] && cz >= 0 && cz < gr.g[2]) {
             const int64_t c = ((int64_t)cz * gr.g[1] + cy) * gr.g[0] + cx;
-            pb = cell_start[c];
-            pe = cell_start[c + 1];
+            pb = cstart[c];
+            pe = cstart[c + 1];
           }
         }
         // lock-step scan of each lane's cell; the valid part of a cell is a prefix (indices ascending)
@@ -340,7 +409,7 @@ __global__ void knn_grid_kernel(const double* __restrict__ coords, const int32_t
       const double reach = (double)r * gr.hmin * (1. - 1e-9);
       if (ts < reach * reach) break;
     }
-    knn_finish<KS>(i, lane, m, d, top, csum, nn + (i - row0) * m, flagged, nflag);
+    knn_finish<KS>(i, lane, m, width, d, top, csum, nn + (i - row0) * width, flagged, nflag);
   }
 }
 
@@ -525,6 +594,153 @@ inline int knn_vecchia_search(const double* coords_dev, const double* coords_hos
   }
   cudaFree(pos_dev); cudaFree(sort_sum_dev); cudaFree(csum_dev);
   return rc;
+}
+
+// The search over independent realizations. Points 0..n_obs-1 are the observed points, cluster by cluster (cluster c: ids
+// [obs_start[c], obs_start[c + 1])); training (pred_start == nullptr) queries all of them, with na = n_obs. Prediction: points
+// n_obs..na-1 are the prediction points, those of cluster c at [pred_start[c], pred_start[c + 1]) (ascending, in the reference's
+// order of the cluster's prediction points), and the ones behind pred_start[K] belong to no cluster with observed points: their rows
+// are all -1 (the prior). Within cluster c the coordinate sums of its observed points, followed by those of its prediction points,
+// are ranked by the same std::sort call the reference makes on that cluster's array. nn_dev: (na - q_begin) x width int32.
+// Why one search, with a grid per large cluster and brute force for the others: with 10^4 clusters of 100 points a query has 100
+// candidates, so a warp scans them faster than it could walk cells, and a search per cluster would cost 10^4 x 8 launches; one
+// shared grid would put a cluster's few points among all the others' in every cell, so a query would scan ~K times more cells.
+inline int knn_cluster_search(const double* coords_dev, const double* coords_host, int64_t na, int64_t n_obs, int d, int width, int m,
+                              int K, const int64_t* obs_start, const int64_t* pred_start, int32_t* nn_dev, cudaStream_t stream,
+                              int num_sms, KnnInfo* info, std::string* err) {
+  const bool pred = pred_start != nullptr;
+  const int64_t q_begin = pred ? n_obs : 0;
+  std::vector<double> csum((size_t)na);
+  for (int64_t i = 0; i < na; ++i) {
+    double sacc = 0.;
+    for (int k = 0; k < d; ++k) sacc += coords_host[i * d + k];
+    csum[(size_t)i] = sacc;
+  }
+  std::vector<KnnClu> clus((size_t)K);
+  std::vector<int32_t> clu_of((size_t)na, -1), loc_of((size_t)na, 0), sort_sum((size_t)na), pos((size_t)na, 0);
+  int64_t seg = 0, ncell = 0;
+  for (int c = 0; c < K; ++c) {
+    KnnClu& C = clus[(size_t)c];
+    C.cand_lo = obs_start[c];
+    C.ncand = obs_start[c + 1] - obs_start[c];
+    const int64_t npc = pred ? pred_start[c + 1] - pred_start[c] : 0;
+    // find_nearest_neighbors_Vecchia_fast caps num_neighbors at end_search_at + 1: the cluster's size - 1 (training), its number of
+    // observed points (prediction)
+    C.m = (int)std::max<int64_t>(0, std::min<int64_t>(m, pred ? C.ncand : C.ncand - 1));
+    C.seg_lo = seg;
+    C.seg_end = seg + C.ncand + npc;
+    std::vector<int> ids((size_t)(C.ncand + npc));
+    for (int64_t l = 0; l < C.ncand; ++l) ids[(size_t)l] = (int)(C.cand_lo + l);
+    for (int64_t l = 0; l < npc; ++l) ids[(size_t)(C.ncand + l)] = (int)(pred_start[c] + l);
+    std::vector<double> cs(ids.size());
+    for (size_t l = 0; l < ids.size(); ++l) { cs[l] = csum[(size_t)ids[l]]; clu_of[(size_t)ids[l]] = c; loc_of[(size_t)ids[l]] = (int32_t)l; }
+    std::vector<int> order(ids.size());
+    std::iota(order.begin(), order.end(), 0);
+    std::sort(order.begin(), order.end(), [&cs](int i1, int i2) { return cs[i1] < cs[i2]; });
+    for (size_t r = 0; r < order.size(); ++r) {
+      sort_sum[(size_t)(seg + (int64_t)r)] = ids[(size_t)order[r]];
+      pos[(size_t)ids[(size_t)order[r]]] = (int32_t)(seg + (int64_t)r);
+    }
+    seg = C.seg_end;
+    C.grid = -1; C.cell_off = 0; C.brute_end = 0;
+    C.gr = KnnGrid();
+    const int64_t be = knn_brute_end(C.ncand, d, C.ncand - 1);
+    if (be < C.ncand && C.m > 0) {
+      C.grid = 1;
+      C.brute_end = be;
+      C.cell_off = ncell;
+      ncell += knn_grid_setup(coords_host + C.cand_lo * d, C.ncand, d, &C.gr);
+    }
+  }
+  for (int64_t i = seg; i < na; ++i) { sort_sum[(size_t)i] = (int32_t)i; pos[(size_t)i] = (int32_t)i; }  // points of no cluster
+  info->ncell = ncell;
+  info->brute_end = na;
+  if (ncell + 1 >= ((int64_t)1 << 31)) { *err = "cell grid too large"; return -1; }
+  int32_t *pos_dev = nullptr, *sort_sum_dev = nullptr, *clu_dev = nullptr, *loc_dev = nullptr, *flagged = nullptr, *nflag = nullptr;
+  double* csum_dev = nullptr;
+  KnnClu* clus_dev = nullptr;
+  uint32_t *cell = nullptr, *cell_sorted = nullptr;
+  int32_t *idx = nullptr, *idx_sorted = nullptr, *cell_start = nullptr;
+  void* tmp = nullptr;
+  int launches = 0;
+  auto ck = [&](cudaError_t e, const char* what) {
+    if (e != cudaSuccess) { *err = std::string(what) + ": " + cudaGetErrorString(e); return false; }
+    return true;
+  };
+  bool ok = ck(cudaMalloc(&pos_dev, sizeof(int32_t) * na), "cudaMalloc") && ck(cudaMalloc(&sort_sum_dev, sizeof(int32_t) * na), "cudaMalloc") &&
+            ck(cudaMalloc(&clu_dev, sizeof(int32_t) * na), "cudaMalloc") && ck(cudaMalloc(&loc_dev, sizeof(int32_t) * na), "cudaMalloc") &&
+            ck(cudaMalloc(&csum_dev, sizeof(double) * na), "cudaMalloc") &&
+            ck(cudaMalloc(&clus_dev, sizeof(KnnClu) * std::max(K, 1)), "cudaMalloc") &&
+            ck(cudaMalloc(&flagged, sizeof(int32_t) * na), "cudaMalloc") && ck(cudaMalloc(&nflag, sizeof(int)), "cudaMalloc");
+  if (ok) ok = ck(cudaMemcpy(pos_dev, pos.data(), sizeof(int32_t) * na, cudaMemcpyHostToDevice), "upload") &&
+               ck(cudaMemcpy(sort_sum_dev, sort_sum.data(), sizeof(int32_t) * na, cudaMemcpyHostToDevice), "upload") &&
+               ck(cudaMemcpy(clu_dev, clu_of.data(), sizeof(int32_t) * na, cudaMemcpyHostToDevice), "upload") &&
+               ck(cudaMemcpy(loc_dev, loc_of.data(), sizeof(int32_t) * na, cudaMemcpyHostToDevice), "upload") &&
+               ck(cudaMemcpy(csum_dev, csum.data(), sizeof(double) * na, cudaMemcpyHostToDevice), "upload") &&
+               ck(cudaMemcpy(clus_dev, clus.data(), sizeof(KnnClu) * K, cudaMemcpyHostToDevice), "upload") &&
+               ck(cudaMemsetAsync(nflag, 0, sizeof(int), stream), "memset");
+  const bool two = width > 32;
+  if (ok) {
+    const int blocks = (int)std::min<int64_t>((na - q_begin + 7) / 8, (int64_t)num_sms * 8);
+    if (two) knn_brute_kernel<2, true><<<std::max(blocks, 1), 256, 0, stream>>>(coords_dev, pos_dev, csum_dev, d, width, q_begin, na, n_obs - 1, q_begin,
+                                                                              nn_dev, flagged, nflag, clus_dev, clu_dev, loc_dev);
+    else knn_brute_kernel<1, true><<<std::max(blocks, 1), 256, 0, stream>>>(coords_dev, pos_dev, csum_dev, d, width, q_begin, na, n_obs - 1, q_begin,
+                                                                          nn_dev, flagged, nflag, clus_dev, clu_dev, loc_dev);
+    ok = ck(cudaGetLastError(), "knn_brute_kernel");
+    ++launches;
+  }
+  if (ok && ncell > 0) {
+    size_t tmp_bytes = 0;
+    ok = ck(cudaMalloc(&cell, sizeof(uint32_t) * na), "cudaMalloc") && ck(cudaMalloc(&cell_sorted, sizeof(uint32_t) * na), "cudaMalloc") &&
+         ck(cudaMalloc(&idx, sizeof(int32_t) * na), "cudaMalloc") && ck(cudaMalloc(&idx_sorted, sizeof(int32_t) * na), "cudaMalloc") &&
+         ck(cudaMalloc(&cell_start, sizeof(int32_t) * (ncell + 1)), "cudaMalloc");
+    if (ok) {
+      knn_cell_id_kernel<<<num_sms * 8, 256, 0, stream>>>(coords_dev, na, KnnGrid(), cell, idx, clus_dev, clu_dev, (uint32_t)ncell);
+      ok = ck(cudaGetLastError(), "knn_cell_id_kernel");
+      ++launches;
+    }
+    int bits = 1;
+    while (((int64_t)1 << bits) <= ncell) ++bits;  // the sentinel cell ncell included
+    if (ok) ok = ck(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cell, cell_sorted, idx, idx_sorted, (int)na, 0, bits, stream), "cub size");
+    if (ok) ok = ck(cudaMalloc(&tmp, tmp_bytes), "cudaMalloc");
+    if (ok) {
+      ok = ck(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, cell, cell_sorted, idx, idx_sorted, (int)na, 0, bits, stream), "cub sort");
+      launches += 4;
+    }
+    if (ok) {
+      knn_cell_start_kernel<<<num_sms * 8, 256, 0, stream>>>(cell_sorted, na, ncell, cell_start);
+      ok = ck(cudaGetLastError(), "knn_cell_start_kernel");
+      ++launches;
+    }
+    if (ok) {
+      KnnGrid g0 = clus[0].gr;
+      g0.dim = d;
+      if (two) knn_grid_kernel<2, true><<<num_sms * 16, 128, 0, stream>>>(coords_dev, pos_dev, csum_dev, cell_start, idx_sorted, g0, width, q_begin, na,
+                                                                         n_obs - 1, q_begin, nn_dev, flagged, nflag, clus_dev, clu_dev, loc_dev);
+      else knn_grid_kernel<1, true><<<num_sms * 16, 128, 0, stream>>>(coords_dev, pos_dev, csum_dev, cell_start, idx_sorted, g0, width, q_begin, na,
+                                                                     n_obs - 1, q_begin, nn_dev, flagged, nflag, clus_dev, clu_dev, loc_dev);
+      ok = ck(cudaGetLastError(), "knn_grid_kernel");
+      ++launches;
+    }
+  }
+  if (ok) {
+    if (two) knn_walk_kernel<2, true><<<num_sms * 4, 128, 0, stream>>>(coords_dev, csum_dev, sort_sum_dev, pos_dev, na, d, width, n_obs - 1, q_begin,
+                                                                      flagged, nflag, nn_dev, clus_dev, clu_dev, loc_dev);
+    else knn_walk_kernel<1, true><<<num_sms * 4, 128, 0, stream>>>(coords_dev, csum_dev, sort_sum_dev, pos_dev, na, d, width, n_obs - 1, q_begin,
+                                                                  flagged, nflag, nn_dev, clus_dev, clu_dev, loc_dev);
+    ok = ck(cudaGetLastError(), "knn_walk_kernel");
+    ++launches;
+    int nf = 0;
+    if (ok) ok = ck(cudaMemcpyAsync(&nf, nflag, sizeof(int), cudaMemcpyDeviceToHost, stream), "memcpy");
+    if (ok) ok = ck(cudaStreamSynchronize(stream), "knn sync");
+    info->replayed = nf;
+  }
+  info->launches = launches;
+  cudaStreamSynchronize(stream);
+  cudaFree(pos_dev); cudaFree(sort_sum_dev); cudaFree(clu_dev); cudaFree(loc_dev); cudaFree(csum_dev); cudaFree(clus_dev);
+  cudaFree(flagged); cudaFree(nflag);
+  cudaFree(cell); cudaFree(cell_sorted); cudaFree(idx); cudaFree(idx_sorted); cudaFree(cell_start); cudaFree(tmp);
+  return ok ? launches : -1;
 }
 
 }  // namespace gpb

@@ -131,6 +131,8 @@ Booster::Booster(const Dataset* train, const char* parameters, REModel* re_model
     Fatal("leaves_newton_update can only be 'true' if Gaussian process boosting is done ");  // c_api.cpp:226-228
   line_search_step_length_ = params_.GetBool("line_search_step_length", false);
   if (line_search_step_length_ && re_model_ == nullptr) line_search_step_length_ = false;  // gbdt.cpp:480: only with a GP model
+  if (line_search_step_length_ && re_model_->IsClustered())
+    Fatal("line_search_step_length is not supported with multiple independent realizations ('cluster_ids') by the CUDA engine yet");
   gpbdev_tree_config cfg;
   cfg.num_leaves = num_leaves_;
   cfg.min_data_in_leaf = params_.GetInt("min_data_in_leaf", 20, {"min_data_per_leaf", "min_data", "min_child_samples"});

@@ -201,10 +201,10 @@ int GPB_SetPredictionData(REModelHandle handle, int32_t num_data_pred, const int
                           const double* covariate_data_pred, const char* vecchia_pred_type, int num_neighbors_pred, double /*cg_delta_conv_pred*/,
                           int /*nsim_var_pred*/, int /*rank_pred_approx_matrix_lanczos*/) {
   API_BEGIN();
-  if (cluster_ids_data_pred != nullptr || re_group_data_pred != nullptr || re_group_rand_coef_data_pred != nullptr ||
-      gp_rand_coef_data_pred != nullptr)
+  if (re_group_data_pred != nullptr || re_group_rand_coef_data_pred != nullptr || gp_rand_coef_data_pred != nullptr)
     throw std::runtime_error("GPB_SetPredictionData: only GP coordinates and covariates are supported as prediction data by this build");
-  M(handle)->SetPredictionData(num_data_pred, gp_coords_data_pred, covariate_data_pred, vecchia_pred_type, num_neighbors_pred);
+  M(handle)->SetPredictionData(num_data_pred, gp_coords_data_pred, covariate_data_pred, vecchia_pred_type, num_neighbors_pred,
+                               cluster_ids_data_pred);
   API_END();
 }
 
@@ -216,11 +216,10 @@ int GPB_PredictREModel(REModelHandle handle, const double* y_data, int32_t num_d
                        const double* /*fixed_effects_pred*/) {
   API_BEGIN();
   if (sample_posterior || sample_prior) throw std::runtime_error("GPB_PredictREModel: posterior / prior sampling is not supported by this build");
-  if (cluster_ids_data_pred != nullptr || re_group_data_pred != nullptr || re_group_rand_coef_data_pred != nullptr ||
-      gp_rand_coef_data_pred != nullptr)
+  if (re_group_data_pred != nullptr || re_group_rand_coef_data_pred != nullptr || gp_rand_coef_data_pred != nullptr)
     throw std::runtime_error("GPB_PredictREModel: only GP coordinates and covariates are supported as prediction data by this build");
   M(handle)->Predict(y_data, num_data_pred, out_predict, predict_cov_mat, predict_var, predict_response, gp_coords_data_pred, cov_pars,
-                     use_saved_data, fixed_effects, covariate_data_pred);
+                     use_saved_data, fixed_effects, covariate_data_pred, cluster_ids_data_pred);
   API_END();
 }
 

@@ -76,12 +76,12 @@ class REModel {
   // GPB_SetPredictionData (c_api.h:1601-1613): prediction locations / neighbour count kept for later Predict calls
   // covariate_data_pred: num_data_pred x num_covariates column-major, required exactly when the model has covariates
   void SetPredictionData(int32_t num_data_pred, const double* gp_coords_data_pred, const double* covariate_data_pred,
-                         const char* vecchia_pred_type, int num_neighbors_pred);
+                         const char* vecchia_pred_type, int num_neighbors_pred, const int32_t* cluster_ids_pred = nullptr);
   // REModel::Predict (re_model.cpp:1081-1215) for the Gaussian Vecchia model (SURVEY §8 f1): out_predict = mean (num_data_pred),
   // followed by the predictive variances when predict_var. gp_coords_data_pred column-major like every matrix of the API.
   void Predict(const double* y_obs, int32_t num_data_pred, double* out_predict, bool predict_cov_mat, bool predict_var,
                bool predict_response, const double* gp_coords_data_pred, const double* cov_pars_pred, bool use_saved_data,
-               const double* fixed_effects, const double* covariate_data_pred = nullptr);
+               const double* fixed_effects, const double* covariate_data_pred = nullptr, const int32_t* cluster_ids_pred = nullptr);
   // Validation data of the boosting loop (RegressionMetric::Eval -> REModel::Predict(use_saved_data, suppress_calc_cov_factor),
   // regression_metric.hpp:92-104, :427-440): the GP's prediction at the locations of GPB_SetPredictionData from the engine's current
   // response (F - y after every boosting iteration: the caller has run one) at the current covariance parameters. The prediction set (locations and neighbour
@@ -110,6 +110,8 @@ class REModel {
   bool IsAnisotropic() const { return aniso_; }
   gpbdev_vecchia_t Engine() const { return engine_; }
   bool IsGrouped() const { return grouped_ != nullptr || gmulti_ != nullptr; }
+  // several independent realizations (cluster_ids with more than one label)
+  bool IsClustered() const { return clustered_; }
   // transformed <-> original scale (cov_fcts.h:485-623)
   void TransformCovPars(const double* orig, double* trans) const;
   void TransformBackCovPars(const double* trans, double* orig) const;
@@ -159,6 +161,13 @@ class REModel {
   int num_cov_pars_ = 3;
   std::mt19937 rng_;
   std::vector<int32_t> perm_;            // ordered position -> original index (data_indices_per_cluster_)
+  // independent realizations (cluster_ids): labels in order of first appearance ({0} without cluster_ids); with more than one
+  // (clustered_) the engine's rows are cluster-major, cluster c at [cluster_start_[c], cluster_start_[c + 1])
+  std::vector<int32_t> cluster_labels_;
+  bool clustered_ = false;
+  std::vector<int64_t> cluster_start_;
+  std::vector<int32_t> cluster_ids_pred_saved_;  // GPB_SetPredictionData's labels (empty: none given)
+  std::vector<int32_t> PredClusters(int32_t num_data_pred, const int32_t* cluster_ids_pred) const;
   std::vector<double> coords_ordered_;   // n x d row-major
   gpbdev_vecchia_t engine_ = nullptr;
   gpbdev_grouped_t grouped_ = nullptr;   // single-level grouped random effect backend (SURVEY §8 a7)

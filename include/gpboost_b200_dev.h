@@ -54,6 +54,14 @@ GPBDEV_EXPORT int gpbdev_vecchia_create(gpbdev_vecchia_t* out, int device, int64
                                         const double* coords_ordered, const int32_t* perm,
                                         const int32_t* nn, int64_t row_begin, int64_t row_end);
 GPBDEV_EXPORT int gpbdev_vecchia_free(gpbdev_vecchia_t h);
+/* Several independent realizations of the GP (cluster_ids; Psi is block diagonal): cluster c holds the ordered rows
+ * [cluster_start[c], cluster_start[c + 1]) (num_clusters + 1 offsets from 0 to n, every cluster non-empty), in the cluster order and
+ * per-cluster Vecchia order of the caller. The device search finds every row's neighbours among the earlier rows of its own cluster
+ * (find_nearest_neighbors_Vecchia_fast per cluster, Vecchia_utils.cpp:1129-1184): the first rows of a cluster take all its earlier
+ * rows, a cluster of c rows keeps at most c - 1 neighbours, and the rows are -1 padded to m. Every pass then runs unchanged on the
+ * padded table. Whole-model engines only. */
+GPBDEV_EXPORT int gpbdev_vecchia_create_clusters(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, const double* coords_ordered,
+                                                 const int32_t* perm, int num_clusters, const int64_t* cluster_start);
 /* The same engine without neighbour sets: for anisotropic kernels, whose sets are searched in the space scaled by covariance
  * parameters (gpbdev_vecchia_search_neighbors), never at creation. Every pass fails until the first search. */
 GPBDEV_EXPORT int gpbdev_vecchia_create_unsearched(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m,
@@ -76,6 +84,8 @@ GPBDEV_EXPORT int gpbdev_vecchia_eval_grad_aniso(gpbdev_vecchia_t h, int cov_typ
 
 /* copy the neighbour sets back (n x m int32, -1 padded) — parity tests */
 GPBDEV_EXPORT int gpbdev_vecchia_get_nn(gpbdev_vecchia_t h, int32_t* nn_host);
+/* copy the ordering back (n int32: ordered row i holds original observation perm[i]) — parity tests */
+GPBDEV_EXPORT int gpbdev_vecchia_get_perm(gpbdev_vecchia_t h, int32_t* perm_host);
 
 /* y in ORIGINAL observation order; host pointer (H2D inside) or device pointer. Replaces SetY
  * (re_model_template.h:6185-6200) incl. the per-cluster re-ordering. */
@@ -129,6 +139,15 @@ GPBDEV_EXPORT int gpbdev_vecchia_predset_create(gpbdev_vecchia_t h, const double
 GPBDEV_EXPORT int gpbdev_vecchia_predset_eval(gpbdev_vecchia_predset_t ps, int cov_type, double var, double range, const double** mean_dev,
                                               const double** var_dev);
 GPBDEV_EXPORT int gpbdev_vecchia_predset_free(gpbdev_vecchia_predset_t ps);
+/* The same for an engine of gpbdev_vecchia_create_clusters (or any engine, as one cluster): cluster_of_pred[p] = the engine's cluster of
+ * prediction point p, or -1 for a cluster without observed points. A point's neighbours are searched among the observed points of its
+ * cluster (at most min(num_neighbors_pred, that cluster's size)); a point of cluster -1 gets mean 0 and D_p = var, the prior. Results
+ * (eval, predict) are in the caller's point order. */
+GPBDEV_EXPORT int gpbdev_vecchia_predset_create_clusters(gpbdev_vecchia_t h, const double* coords_pred_host, int64_t np, int num_neighbors_pred,
+                                                         const int32_t* cluster_of_pred, gpbdev_vecchia_predset_t* out);
+GPBDEV_EXPORT int gpbdev_vecchia_predict_clusters(gpbdev_vecchia_t h, int cov_type, double var, double range, const double* coords_pred_host,
+                                                  int64_t np, int num_neighbors_pred, const int32_t* cluster_of_pred, double* mean_out_host,
+                                                  double* var_out_host);
 /* Newton update of the leaf values in GPBoost (SURVEY §8 f2; REModelTemplate::NewtonUpdateLeafValues, Vecchia branch,
  * include/GPBoost/re_model_template.h:4982-5063). After a STORE pass at the current parameters: M_host (L x L row-major) =
  * H^T B^T D^-1 B H and rhs_host (L) = H^T g for the leaf incidence H given by leaf_of_row_dev (n int32, original row order, device)
