@@ -201,6 +201,7 @@ struct gpbdev_vecchia {
   double* flush = nullptr;
   int64_t flush_n = 0;
   int grid_cap = 0;
+  int64_t partial_rows = 0;   // rows of kNumAcc sums that `partials` holds
   int64_t launches = 0;
   bool factor_stored = false;
   // parameters of the stored factor and of the last pass (whose sums sit in `sums`): a STORE request for exactly this state is
@@ -309,6 +310,8 @@ int launch_eval(gpbdev_vecchia* h, int cov_type, double var, double range, int m
   // all-reduce of the sums over the ranks on this stream (NCCL kernel), and the record of a stored factor
   auto finish = [&](int64_t rows) -> int {
     CUDA_TRY(cudaGetLastError());
+    if (rows > h->partial_rows)
+      return fail("gpbdev_vecchia_eval: " + std::to_string(rows) + " partial rows launched, " + std::to_string(h->partial_rows) + " allocated");
     reduce_partials_kernel<<<1, 256, 0, h->stream>>>(h->partials, rows, h->sums);
     CUDA_TRY(cudaGetLastError());
     h->launches += 2;
@@ -454,7 +457,10 @@ int vecchia_create(gpbdev_vecchia_t* out, int device, int64_t n, int d, int m, c
   const int64_t rows = row_end - row_begin;
   const int64_t max_blocks = (rows + gpb::kWarpsPerBlock - 1) / gpb::kWarpsPerBlock;
   if (h->grid_cap > max_blocks) h->grid_cap = (int)std::max<int64_t>(max_blocks, 1);
-  CUDA_TRY(cudaMalloc(&h->partials, sizeof(double) * h->grid_cap * gpb::kWarpsPerBlock * gpb::kNumAcc));
+  // the two-observation kernel launches at least one CTA of kWarpsPerBlock warps with two partial rows each, even on a shard of
+  // at most kWarpsPerBlock rows (grid_cap = 1)
+  h->partial_rows = (int64_t)std::max(h->grid_cap, 2) * gpb::kWarpsPerBlock;
+  CUDA_TRY(cudaMalloc(&h->partials, sizeof(double) * h->partial_rows * gpb::kNumAcc));
   CUDA_TRY(cudaMalloc(&h->sums, sizeof(double) * gpb::kNumAcc));
   CUDA_TRY(cudaMallocHost(&h->sums_host, sizeof(double) * gpb::kNumAcc));
   CUDA_TRY(cudaMallocHost(&h->stage_host, sizeof(double) * n));

@@ -176,3 +176,40 @@ def dense_neg_log_likelihood(coords, cov_pars, y, cov_function="matern", cov_fct
     if rc != 0:
         raise FloatingPointError("dense Cholesky failed")
     return out[0]
+
+
+# ---- long-double per-row reference with error bounds (orc_vecchia_rows_ld)
+ROWS_NOUT = 24
+ROWS_COLS = ["D", "By", "u", "quad", "logD", "t3", "t4", "t5", "t6", "t7", "t8",
+             "bD", "bBy", "bu", "bquad", "blogD", "bt3", "bt4", "bt5", "bt6", "bt7", "bt8", "kappa", "eps"]
+# relative error of one fp64 covariance evaluation (exp to 2 ulp, the Matern polynomial, the products) and of one distance (d
+# rounded squares summed, the square root, the pre-scaling by the range) in units of u = 2^-53: the c_v and c_r of the bound
+COV_EVAL_ULPS = 8.
+
+
+def dist_ulps(d):
+    return d + 4.
+
+
+def rows_ld(coords, nn_rows, cid, var, range_, diag_nb, diag_obs, y, row_begin=0, qcoords=None, cov_mult=1.0, drop=None):
+    """Rows [row_begin, row_begin + len(nn_rows)) of the Vecchia factor in long double, with first-order bounds of an fp64
+    evaluation (oracle/vecchia_oracle.c: orc_vecchia_rows_ld). coords (n, d) in Vecchia order; nn_rows the neighbour rows of these
+    rows; qcoords (nrows, d): prediction rows (own point = query, y_i = 0; pass diag_obs = var). cov_mult / drop = (row, a, b):
+    deliberate faults. Returns (dict column -> (nrows,) array, A (nrows, m), bound of A (nrows, m), number of bad rows)."""
+    coords = np.asarray(coords, dtype=np.float64)
+    n, d = coords.shape
+    nn_rows = np.ascontiguousarray(nn_rows, dtype=np.int32)
+    nrows, m = nn_rows.shape
+    cm = np.asfortranarray(coords)
+    qc = None if qcoords is None else np.asfortranarray(np.asarray(qcoords, dtype=np.float64).reshape(nrows, d))
+    yy = np.ascontiguousarray(np.zeros(n) if y is None else y, dtype=np.float64)
+    out = np.empty((nrows, ROWS_NOUT)); A = np.empty((nrows, m)); bA = np.empty((nrows, m))
+    dr = None if drop is None else np.ascontiguousarray(drop, dtype=np.int64)
+    L = lib()
+    L.orc_vecchia_rows_ld.restype = C.c_int
+    bad = L.orc_vecchia_rows_ld(
+        _p(cm), C.c_int64(n), C.c_int(d), C.c_int(m), _p(nn_rows, C.c_int32), C.c_int(cid), C.c_double(var), C.c_double(range_),
+        C.c_double(diag_nb), C.c_double(diag_obs), _p(yy), None if qc is None else _p(qc), C.c_int64(row_begin), C.c_int64(nrows),
+        C.c_double(COV_EVAL_ULPS), C.c_double(dist_ulps(d)), C.c_double(cov_mult), None if dr is None else _p(dr, C.c_int64),
+        _p(out), _p(A), _p(bA))
+    return {k: out[:, j] for j, k in enumerate(ROWS_COLS)}, A, bA, bad

@@ -471,3 +471,229 @@ int orc_dense_nll(const double* coords, int n, int d, int cov_type, const double
   free(P); free(z);
   return 0;
 }
+
+/* ==== long-double per-row reference of the Vecchia factor passes, with first-order error bounds of an fp64 evaluation ====
+ * Not a restatement of the reference library: the same row quantities as orc_vecchia_factor / orc_vecchia_nll /
+ * orc_vecchia_grad, evaluated in long double (distances, covariances, Cholesky) from the fp64 inputs, row by row, together
+ * with bounds on what any backward-stable fp64 evaluation of the row may differ from it.
+ *
+ * Row r of [row_begin, row_begin + nrows): own point i = row_begin + r (model row: coords of i, y_i = y[i]) or, when qcoords is
+ * given, query point r of qcoords (prediction row: y_i = 0; the caller passes diag_obs = var). Neighbours nn[r * m + k], -1
+ * entries are skipped wherever they sit. Augmented matrix St = [[S_NN, s], [s^T, diag_obs]] with S_NN's diagonal = diag_nb.
+ *
+ * Entrywise perturbation E of St (u = 2^-53, gam(k) = k u / (1 - k u)):
+ *   off-diagonal  E_ab = u (cv |St_ab| + |dSigma/dr|_ab (cr r_ab + sqrt(d) (|x_a|_inf + |x_b|_inf))) + gam(q + 2) sqrt(St_aa St_bb)
+ *   diagonal      E_aa = u |St_aa| + gam(q + 2) St_aa
+ * (covariance evaluation, distance rounding, rounding of the coordinates themselves, Cholesky backward error). With b = [-A_i, 1]
+ * and wt = [S_NN^-1 y_N, 0]: beta_D = |b|^T E |b|, beta_By = |b|^T E |wt| + gam(q + 2) (|y_i| + |A_i| |y_N|),
+ * beta_A = |S_NN^-1| (E_N. |b|). GRAD terms: kappa (eps + rho) (magnitude of the term with every factor in absolute value),
+ * kappa the 1-norm condition number of S_NN (>= the 2-norm one), eps = max E_ab / sqrt(St_aa St_bb) and rho the largest relative
+ * evaluation error of one covariance (the derivative values carry it too; it dominates for tiny covariances, where eps does not
+ * see it).
+ *
+ * out: nrows x ORC_ROWS_NOUT, columns
+ *   0 D  1 By  2 u = By / D  3 By^2 / D  4 log D  5..10 the GRAD accumulator terms (kNumAcc slots 3..8: u_var u, u_range u,
+ *   u^2 dD_var, u^2 dD_range, dD_var / D, dD_range / D)  11 beta_D  12 beta_By  13 beta_u  14 beta(By^2 / D)  15 beta(log D)
+ *   16..21 bounds of the GRAD terms  22 kappa  23 eps
+ * A, bA: nrows x m (0 at -1 slots). cov_mult scales every covariance (off-diagonal, including s) and drop = {row, a, b} zeroes
+ * the pair (a, b) of the neighbour block of one row (row -1: none): deliberate faults, for tests of the bounds themselves.
+ * Returns the number of rows whose neighbour block is not positive definite. */
+#define ORC_ROWS_NOUT 24
+typedef long double orc_ld;
+
+static orc_ld orc_cov_ld(int type, orc_ld dist, orc_ld var, orc_ld range) {
+  orc_ld rd;
+  switch (type) {
+    case ORC_COV_EXPONENTIAL: return var * expl(-range * dist);
+    case ORC_COV_MATERN15: rd = range * dist; return var * (1.L + rd) * expl(-rd);
+    case ORC_COV_MATERN25: rd = range * dist; return var * (1.L + rd + rd * rd / 3.L) * expl(-rd);
+    default: return var * expl(-range * dist * dist);
+  }
+}
+/* d Sigma / d dist */
+static orc_ld orc_cov_ddist_ld(int type, orc_ld dist, orc_ld var, orc_ld range) {
+  orc_ld rd = range * dist;
+  switch (type) {
+    case ORC_COV_EXPONENTIAL: return -range * var * expl(-rd);
+    case ORC_COV_MATERN15: return -var * range * rd * expl(-rd);
+    case ORC_COV_MATERN25: return -var * range * rd * (1.L + rd) / 3.L * expl(-rd);
+    default: return -2.L * range * dist * var * expl(-range * dist * dist);
+  }
+}
+/* d Sigma / d log range (transformed): dist dSigma/ddist, half of it for the Gaussian kernel (a function of range dist^2) */
+static orc_ld orc_cov_grad_range_ld(int type, orc_ld dist, orc_ld var, orc_ld range) {
+  orc_ld g = dist * orc_cov_ddist_ld(type, dist, var, range);
+  return type == ORC_COV_GAUSSIAN ? 0.5L * g : g;
+}
+
+static int orc_chol_ld(orc_ld* a, int q, int ld) {
+  for (int j = 0; j < q; ++j) {
+    orc_ld s = a[j * ld + j];
+    for (int k = 0; k < j; ++k) s -= a[j * ld + k] * a[j * ld + k];
+    if (!(s > 0.L)) return -1;
+    orc_ld l = sqrtl(s);
+    a[j * ld + j] = l;
+    for (int i = j + 1; i < q; ++i) {
+      orc_ld t = a[i * ld + j];
+      for (int k = 0; k < j; ++k) t -= a[i * ld + k] * a[j * ld + k];
+      a[i * ld + j] = t / l;
+    }
+  }
+  return 0;
+}
+static void orc_chol_solve_ld(const orc_ld* l, int q, int ld, orc_ld* b) {
+  for (int i = 0; i < q; ++i) {
+    orc_ld t = b[i];
+    for (int k = 0; k < i; ++k) t -= l[i * ld + k] * b[k];
+    b[i] = t / l[i * ld + i];
+  }
+  for (int i = q - 1; i >= 0; --i) {
+    orc_ld t = b[i];
+    for (int k = i + 1; k < q; ++k) t -= l[k * ld + i] * b[k];
+    b[i] = t / l[i * ld + i];
+  }
+}
+
+int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int32_t* nn, int cov_type, double var_d,
+                        double range_d, double diag_nb, double diag_obs, const double* y, const double* qcoords, int64_t row_begin,
+                        int64_t nrows, double cv, double cr, double cov_mult, const int64_t* drop, double* out, double* A,
+                        double* bA) {
+  const orc_ld u = ldexpl(1.L, -53), var = var_d, range = range_d, mult = cov_mult;
+  const int M = m + 1;
+  int bad = 0;
+#pragma omp parallel
+  {
+    orc_ld* x = (orc_ld*)malloc(sizeof(orc_ld) * M * d);  /* points: neighbours 0..q-1, own point q */
+    orc_ld* xn = (orc_ld*)malloc(sizeof(orc_ld) * M);     /* |x|_inf */
+    orc_ld* St = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* E = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* G0 = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* G1 = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* L = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* Si = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* a = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* w = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* yn = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* t = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    int* pos = (int*)malloc(sizeof(int) * M);
+#pragma omp for schedule(dynamic, 64) reduction(+ : bad)
+    for (int64_t r = 0; r < nrows; ++r) {
+      const int64_t i = row_begin + r;
+      const int32_t* nb = nn + (size_t)r * m;
+      double* o = out + (size_t)r * ORC_ROWS_NOUT;
+      for (int k = 0; k < m; ++k) { A[(size_t)r * m + k] = 0.; bA[(size_t)r * m + k] = 0.; }
+      int q = 0;
+      for (int k = 0; k < m; ++k)
+        if (nb[k] >= 0) pos[q++] = k;
+      for (int c = 0; c < d; ++c) {
+        for (int j = 0; j < q; ++j) x[j * d + c] = coords[(size_t)c * n + nb[pos[j]]];
+        x[q * d + c] = qcoords ? qcoords[(size_t)c * nrows + r] : coords[(size_t)c * n + i];
+      }
+      for (int j = 0; j <= q; ++j) {
+        orc_ld mx = 0.L;
+        for (int c = 0; c < d; ++c) mx = fmaxl(mx, fabsl(x[j * d + c]));
+        xn[j] = mx;
+        yn[j] = j < q ? (orc_ld)y[nb[pos[j]]] : (qcoords ? 0.L : (orc_ld)y[i]);
+      }
+      const orc_ld gam = (q + 2) * u / (1.L - (q + 2) * u);
+      orc_ld rho = 0.L; /* largest relative evaluation error of one covariance */
+      for (int p = 0; p <= q; ++p) {
+        St[p * M + p] = p < q ? (orc_ld)diag_nb : (orc_ld)diag_obs;
+        G0[p * M + p] = var;
+        G1[p * M + p] = 0.L;
+        for (int s = p + 1; s <= q; ++s) {
+          orc_ld r2 = 0.L;
+          for (int c = 0; c < d; ++c) { orc_ld df = x[p * d + c] - x[s * d + c]; r2 += df * df; }
+          const orc_ld dist = sqrtl(r2);
+          orc_ld c0 = orc_cov_ld(cov_type, dist, var, range);
+          const orc_ld dd = orc_cov_ddist_ld(cov_type, dist, var, range);
+          G0[p * M + s] = G0[s * M + p] = c0;
+          G1[p * M + s] = G1[s * M + p] = orc_cov_grad_range_ld(cov_type, dist, var, range);
+          c0 *= mult;
+          if (drop && drop[0] == r && ((drop[1] == p && drop[2] == s) || (drop[1] == s && drop[2] == p))) c0 = 0.L;
+          St[p * M + s] = St[s * M + p] = c0;
+          E[p * M + s] = E[s * M + p] =
+              u * (cv * fabsl(c0) + fabsl(dd) * (cr * dist + sqrtl((orc_ld)d) * (xn[p] + xn[s])));
+          if (c0 != 0.L) rho = fmaxl(rho, E[p * M + s] / fabsl(c0));
+        }
+      }
+      orc_ld eps = 0.L;
+      for (int p = 0; p <= q; ++p) {
+        E[p * M + p] = u * fabsl(St[p * M + p]) + gam * St[p * M + p];
+        for (int s = 0; s < p; ++s) {
+          const orc_ld sc = sqrtl(St[p * M + p] * St[s * M + s]);
+          E[p * M + s] += gam * sc;
+          E[s * M + p] = E[p * M + s];
+        }
+        for (int s = 0; s <= p; ++s) eps = fmaxl(eps, E[p * M + s] / sqrtl(St[p * M + p] * St[s * M + s]));
+      }
+      for (int p = 0; p < q; ++p)
+        for (int s = 0; s < q; ++s) L[p * M + s] = St[p * M + s];
+      if (orc_chol_ld(L, q, M) != 0) { ++bad; for (int k = 0; k < ORC_ROWS_NOUT; ++k) o[k] = NAN; continue; }
+      for (int p = 0; p < q; ++p) { a[p] = St[p * M + q]; w[p] = yn[p]; }
+      orc_chol_solve_ld(L, q, M, a);
+      orc_chol_solve_ld(L, q, M, w);
+      for (int c = 0; c < q; ++c) { /* S_NN^-1, column c */
+        for (int p = 0; p < q; ++p) t[p] = p == c ? 1.L : 0.L;
+        orc_chol_solve_ld(L, q, M, t);
+        for (int p = 0; p < q; ++p) Si[p * M + c] = t[p];
+      }
+      orc_ld D = St[q * M + q], By = yn[q];
+      for (int p = 0; p < q; ++p) { D -= a[p] * St[p * M + q]; By -= a[p] * yn[p]; }
+      if (!(D > 0.L)) ++bad;
+      const orc_ld uu = By / D;
+      /* b = [-a, 1], wt = [w, 0] */
+      a[q] = -1.L; w[q] = 0.L;
+      orc_ld bD = 0.L, bBy = 0.L, ay = fabsl(yn[q]);
+      for (int p = 0; p <= q; ++p) {
+        orc_ld eb = 0.L;
+        for (int s = 0; s <= q; ++s) eb += E[p * M + s] * fabsl(a[s]);
+        bD += fabsl(a[p]) * eb;
+        bBy += fabsl(w[p]) * eb;
+        t[p] = eb;
+        if (p < q) ay += fabsl(a[p] * yn[p]);
+      }
+      bBy += gam * ay;
+      for (int p = 0; p < q; ++p) {
+        orc_ld s = 0.L;
+        for (int c = 0; c < q; ++c) s += fabsl(Si[p * M + c]) * t[c];
+        A[(size_t)r * m + pos[p]] = (double)a[p];
+        bA[(size_t)r * m + pos[p]] = (double)s;
+      }
+      orc_ld n1 = 0.L, ni = 0.L; /* kappa_1 = |S|_1 |S^-1|_1 */
+      for (int c = 0; c < q; ++c) {
+        orc_ld s1 = 0.L, s2 = 0.L;
+        for (int p = 0; p < q; ++p) { s1 += fabsl(St[p * M + c]); s2 += fabsl(Si[p * M + c]); }
+        n1 = fmaxl(n1, s1); ni = fmaxl(ni, s2);
+      }
+      const orc_ld kap = q > 0 ? n1 * ni : 1.L, ke = kap * (eps + rho);
+      const orc_ld bu = bBy / D + fabsl(By) * bD / (D * D), Mu = ay / D;
+      o[0] = (double)D; o[1] = (double)By; o[2] = (double)uu; o[3] = (double)(By * By / D); o[4] = (double)logl(D);
+      o[11] = (double)bD; o[12] = (double)bBy; o[13] = (double)bu;
+      o[14] = (double)(2.L * fabsl(By) * bBy / D + By * By * bD / (D * D) + 3.L * u * By * By / D);
+      o[15] = (double)(bD / D + u * (1.L + fabsl(logl(D))));
+      o[22] = (double)kap; o[23] = (double)eps;
+      for (int k = 0; k < 2; ++k) { /* u_k = -(g - G_NN A).(S_NN^-1 y_N), dD_k = G_qq - 2 A.g + A^T G_NN A (g = G_Nq) */
+        const orc_ld* G = k == 0 ? G0 : G1;
+        orc_ld uk = 0.L, Muk = 0.L, dD = G[q * M + q], MdD = fabsl(G[q * M + q]);
+        for (int p = 0; p < q; ++p) {
+          orc_ld ga = 0.L, gaa = 0.L;
+          for (int s = 0; s < q; ++s) { ga += G[p * M + s] * a[s]; gaa += fabsl(G[p * M + s] * a[s]); }
+          const orc_ld g = G[p * M + q];
+          uk -= (g - ga) * w[p];
+          Muk += (fabsl(g) + gaa) * fabsl(w[p]);
+          dD += -2.L * a[p] * g + a[p] * ga;
+          MdD += 2.L * fabsl(a[p] * g) + fabsl(a[p]) * gaa;
+        }
+        o[5 + k] = (double)(uk * uu);
+        o[7 + k] = (double)(uu * uu * dD);
+        o[9 + k] = (double)(dD / D);
+        o[16 + k] = (double)(ke * (Muk * fabsl(uu) + fabsl(uk) * Mu));
+        o[18 + k] = (double)(ke * (uu * uu * MdD + 2.L * fabsl(uu) * Mu * fabsl(dD)));
+        o[20 + k] = (double)(ke * (MdD + fabsl(dD)) / D);
+      }
+    }
+    free(x); free(xn); free(St); free(E); free(G0); free(G1); free(L); free(Si); free(a); free(w); free(yn); free(t); free(pos);
+  }
+  return bad;
+}
