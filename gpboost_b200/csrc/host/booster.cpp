@@ -9,6 +9,7 @@
 #include <sstream>
 #include <stdexcept>
 
+#include "collective.h"
 #include "runtime.h"
 
 namespace gpb200 {
@@ -147,11 +148,7 @@ Booster::Booster(const Dataset* train, const char* parameters, REModel* re_model
   const Runtime& rt = GetRuntime();
   row_begin_ = 0; row_end_ = n_;
   if (rt.world_size > 1) {
-    if (rt.allreduce_dev == nullptr)
-      Fatal("Boosting over several ranks needs the native collective (GPB200_NcclInit): histograms are all-reduced on the device");
-    const int64_t chunk = (n_ + rt.world_size - 1) / rt.world_size;
-    row_begin_ = std::min<int64_t>(n_, chunk * rt.rank);
-    row_end_ = std::min<int64_t>(n_, row_begin_ + chunk);
+    RowShard(n_, &row_begin_, &row_end_);
     if (row_end_ <= row_begin_) Fatal("More ranks than training rows");
     sharded_ = true;
   }
@@ -160,7 +157,7 @@ Booster::Booster(const Dataset* train, const char* parameters, REModel* re_model
   const int Fpad = train->bins_row_stride();
   TreeCheck(gpbdev_tree_create_on_device_bins(&learner_, rt.device, row_end_ - row_begin_, F, Fpad,
                                               train->bins_device() + (size_t)row_begin_ * Fpad, num_bin.data(), &cfg));
-  if (sharded_) TreeCheck(gpbdev_tree_set_allreduce(learner_, rt.allreduce_dev, rt.allreduce_ctx, n_));
+  if (sharded_) TreeCheck(gpbdev_tree_set_allreduce(learner_, NcclAllReduceSumDevice, nullptr, n_));
   TreeCheck(gpbdev_vec_alloc(learner_, &score_dev_, n_));
   TreeCheck(gpbdev_vec_alloc(learner_, &label_dev_, n_));
   TreeCheck(gpbdev_vec_alloc(learner_, &grad_dev_, n_));

@@ -609,17 +609,6 @@ int GPB200_SetDevice(int device) {
   API_END();
 }
 
-int GPB200_SetCollective(int rank, int world_size, void* allreduce_sum) {
-  API_BEGIN();
-  if (world_size < 1 || rank < 0 || rank >= world_size) throw std::runtime_error("GPB200_SetCollective: bad rank / world_size");
-  if (world_size > 1 && allreduce_sum == nullptr) throw std::runtime_error("GPB200_SetCollective: world_size > 1 needs an all-reduce function");
-  gpb200::Runtime& rt = gpb200::GetRuntime();
-  rt.rank = rank;
-  rt.world_size = world_size;
-  rt.allreduce_sum = reinterpret_cast<gpb200::AllReduceSumFn>(allreduce_sum);
-  API_END();
-}
-
 int GPB200_NcclGetUniqueId(char* id128) {
   API_BEGIN();
   gpb200::NcclGetUniqueId(id128);

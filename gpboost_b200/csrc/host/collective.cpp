@@ -58,20 +58,6 @@ void Check(int rc, const char* what) {
 void CudaCheck(cudaError_t e, const char* what) {
   if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
 }
-
-// host-buffer all-reduce (Runtime::allreduce_sum): staged through a device scratch buffer; used for the handful of
-// scalars the host logic itself owns (e.g. the common SLQ stopping test)
-void HostAllReduce(double* buf, int count) {
-  if ((size_t)count > g.scratch_count) {
-    if (g.scratch) cudaFree(g.scratch);
-    g.scratch_count = std::max<size_t>(1024, (size_t)count);
-    CudaCheck(cudaMalloc(&g.scratch, sizeof(double) * g.scratch_count), "cudaMalloc");
-  }
-  CudaCheck(cudaMemcpyAsync(g.scratch, buf, sizeof(double) * count, cudaMemcpyHostToDevice, g.stream), "H2D");
-  Check(g.AllReduce(g.scratch, g.scratch, (size_t)count, ncclFloat64, ncclSum, g.comm, g.stream), "ncclAllReduce");
-  CudaCheck(cudaMemcpyAsync(buf, g.scratch, sizeof(double) * count, cudaMemcpyDeviceToHost, g.stream), "D2H");
-  CudaCheck(cudaStreamSynchronize(g.stream), "sync");
-}
 }  // namespace
 
 void NcclGetUniqueId(char* id) {
@@ -93,9 +79,6 @@ void NcclInit(int rank, int world_size, const char* id) {
   CudaCheck(cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking), "cudaStreamCreate");
   rt.rank = rank;
   rt.world_size = world_size;
-  rt.allreduce_sum = HostAllReduce;
-  rt.allreduce_dev = NcclAllReduceSumDevice;
-  rt.allreduce_ctx = nullptr;
 }
 
 void NcclFinalize() {
@@ -105,12 +88,31 @@ void NcclFinalize() {
   if (g.stream) { cudaStreamDestroy(g.stream); g.stream = nullptr; }
   if (g.scratch) { cudaFree(g.scratch); g.scratch = nullptr; g.scratch_count = 0; }
   Runtime& rt = GetRuntime();
-  rt.rank = 0; rt.world_size = 1; rt.allreduce_sum = nullptr; rt.allreduce_dev = nullptr;
+  rt.rank = 0; rt.world_size = 1;
 }
 
 int NcclAllReduceSumDevice(void* /*ctx*/, double* buf, int64_t count, void* stream) {
   if (!g.comm) return -1;
   return g.AllReduce(buf, buf, (size_t)count, ncclFloat64, ncclSum, g.comm, reinterpret_cast<cudaStream_t>(stream)) == ncclSuccess ? 0 : -1;
+}
+
+void NcclAllReduceSumHost(double* buf, int count) {
+  if ((size_t)count > g.scratch_count) {
+    if (g.scratch) cudaFree(g.scratch);
+    g.scratch_count = std::max<size_t>(1024, (size_t)count);
+    CudaCheck(cudaMalloc(&g.scratch, sizeof(double) * g.scratch_count), "cudaMalloc");
+  }
+  CudaCheck(cudaMemcpyAsync(g.scratch, buf, sizeof(double) * count, cudaMemcpyHostToDevice, g.stream), "H2D");
+  Check(g.AllReduce(g.scratch, g.scratch, (size_t)count, ncclFloat64, ncclSum, g.comm, g.stream), "ncclAllReduce");
+  CudaCheck(cudaMemcpyAsync(buf, g.scratch, sizeof(double) * count, cudaMemcpyDeviceToHost, g.stream), "D2H");
+  CudaCheck(cudaStreamSynchronize(g.stream), "sync");
+}
+
+void RowShard(int64_t n, int64_t* begin, int64_t* end) {
+  const Runtime& rt = GetRuntime();
+  const int64_t chunk = (n + rt.world_size - 1) / rt.world_size;
+  *begin = std::min<int64_t>(n, chunk * rt.rank);
+  *end = std::min<int64_t>(n, *begin + chunk);
 }
 
 }  // namespace gpb200

@@ -12,6 +12,7 @@
 #include <stdexcept>
 #include <unordered_map>
 
+#include "collective.h"
 #include "runtime.h"
 
 namespace gpb200 {
@@ -258,12 +259,10 @@ REModel::REModel(int32_t num_data, const int32_t* cluster_ids_data, const char* 
     for (int k = 0; k < dim_; ++k) coords_ordered_[(size_t)i * dim_ + k] = gp_coords_data[(size_t)k * num_data_ + perm_[i]];
   // ---- device state (+ device neighbour search)
   const Runtime& rt = GetRuntime();
+  // non-Gaussian: every rank holds the whole factor, the SLQ probe columns are sharded
+  const bool sharded = rt.world_size > 1 && gauss_;
   int64_t rb = 0, re = num_data_;
-  if (rt.world_size > 1 && gauss_) {  // non-Gaussian: every rank holds the whole factor, the SLQ probe columns are sharded
-    const int64_t chunk = (num_data_ + rt.world_size - 1) / rt.world_size;
-    rb = std::min<int64_t>(num_data_, chunk * rt.rank);
-    re = std::min<int64_t>(num_data_, rb + chunk);
-  }
+  if (sharded) RowShard(num_data_, &rb, &re);
   if (clustered_)
     DevCheck(gpbdev_vecchia_create_clusters(&engine_, rt.device, num_data_, dim_, num_neighbors_, coords_ordered_.data(), perm_.data(),
                                             (int)cluster_labels_.size(), cluster_start_.data()));
@@ -273,11 +272,8 @@ REModel::REModel(int32_t num_data, const int32_t* cluster_ids_data, const char* 
   else
     DevCheck(gpbdev_vecchia_create(&engine_, rt.device, num_data_, dim_, num_neighbors_, coords_ordered_.data(), perm_.data(),
                                    nullptr, rb, re));
-  if (rt.world_size > 1 && gauss_ && rt.allreduce_dev != nullptr) {
-    // native collective (GPB200_NcclInit): the engine sums its shard results over the ranks on its own stream
-    DevCheck(gpbdev_vecchia_set_allreduce(engine_, rt.allreduce_dev, rt.allreduce_ctx));
-    device_collective_ = true;
-  }
+  // the engine sums its shard results over the ranks on its own stream
+  if (sharded) DevCheck(gpbdev_vecchia_set_allreduce(engine_, NcclAllReduceSumDevice, nullptr));
   estimate_cov_par_index_.assign(num_cov_pars_, 1);
   std::memset(sums_, 0, sizeof(sums_));
 }
@@ -618,11 +614,6 @@ void REModel::AnisoSetRanges(const double* lambda, bool search) {
 
 void REModel::DevicePass(double var, double range, int mode) {
   DevCheck(gpbdev_vecchia_eval(engine_, cov_id_, var, range, mode, sums_));
-  const Runtime& rt = GetRuntime();
-  if (rt.world_size > 1 && !device_collective_) {
-    if (rt.allreduce_sum == nullptr) Fatal("world_size > 1 but no all-reduce callback was registered (GPB200_SetCollective)");
-    rt.allreduce_sum(sums_, GPBDEV_NUM_SUMS);
-  }
   ++num_ll_evals_;
   if (sums_[GPBDEV_SUM_NBAD] > 0.) {
     // Vecchia_utils.cpp:1685-1698: warning for Gaussian likelihoods; the likelihood becomes NaN/Inf and the
@@ -701,10 +692,7 @@ void REModel::EnsureProbes() {
   DrawProbes(seed_rand_vec_trace_, cg_generator_counter_, num_data_, cols, probes.data());
   ++cg_generator_counter_;
   DevCheck(gpbdev_vecchia_laplace_set_probes(engine_, probes.data(), tl));
-  if (rt.world_size > 1) {
-    if (rt.allreduce_sum == nullptr) Fatal("world_size > 1 but no all-reduce callback was registered (GPB200_SetCollective)");
-    DevCheck(gpbdev_vecchia_laplace_set_collective(engine_, rt.allreduce_sum, t));
-  }
+  if (rt.world_size > 1) DevCheck(gpbdev_vecchia_laplace_set_collective(engine_, NcclAllReduceSumHost, t));
   probes_t_ = t;
   probes_seed_ = seed_rand_vec_trace_;
 }
@@ -1121,9 +1109,9 @@ void REModel::OptimCovParLaplace(const double* y_data, const double* fixed_effec
 
 bool REModel::DevicePathReady() const {
   // initial covariance parameters come from the sample variance of the response (FindInitCovPar): the first call takes the
-  // host-pointer form; the dense backend and an injected host collective have no device-resident entry
+  // host-pointer form; the dense backend has no device-resident entry, and over several processes only a Vecchia model takes it
   const Runtime& rt = GetRuntime();
-  return gauss_ && cov_pars_initialized_ && dense_ == nullptr && !(rt.world_size > 1 && !device_collective_);
+  return gauss_ && cov_pars_initialized_ && dense_ == nullptr && !(rt.world_size > 1 && engine_ == nullptr);
 }
 
 void REModel::SetYDevice(const double* y_dev) {
@@ -1319,8 +1307,6 @@ void REModel::CalcGradient(double* y, const double* fixed_effects, bool /*calc_c
   DevCheck(gpbdev_vecchia_set_y(engine_, y));
   DevicePass(cov_pars_[1], cov_pars_[2], GPBDEV_MODE_STORE);
   DevCheck(gpbdev_vecchia_yaux(engine_, y));
-  const Runtime& rt = GetRuntime();
-  if (rt.world_size > 1 && !device_collective_) rt.allreduce_sum(y, num_data_);
   const double inv_s2 = 1. / cov_pars_[0];
   for (int32_t i = 0; i < num_data_; ++i) y[i] *= inv_s2;
 }

@@ -176,7 +176,6 @@ class REModel {
   // non-Gaussian likelihood (bernoulli_logit, poisson) with a latent Vecchia GP: Laplace approximation on the device (SURVEY §8 a12)
   bool gauss_ = true;
   bool poisson_ = false;
-  bool device_collective_ = false;  // the engine all-reduces its results itself (NCCL on its stream)
   void EvalLaplace(const double* y_data, const double* cov_pars, double* negll, const double* fixed_effects);
   // checks poisson labels (non-negative integers) and returns -sum_i log(y_i!)
   double CheckCountsLogNormConst(const double* y) const;

@@ -206,7 +206,7 @@ GPBDEV_EXPORT int gpbdev_knn_search(int device, const double* coords_host, int64
  * The Vecchia factor kernel is FP64-pipe bound (SURVEY §8d), so this is its roofline denominator. */
 /* Device collective hook (multi-GPU): in-place sum over all ranks of `count` fp64 values at DEVICE pointer `dev_buf`, enqueued on
  * `stream` (cudaStream_t). With a hook installed the engine all-reduces its 9 sums (and the Psi^-1 y vector) on its own stream
- * before they leave the device; without one the caller reduces the host copies (the injected collective of GPB200_SetCollective). */
+ * before they leave the device; without one the caller reduces the host copies. */
 typedef int (*gpbdev_allreduce_fn)(void* ctx, double* dev_buf, int64_t count, void* stream);
 GPBDEV_EXPORT int gpbdev_vecchia_set_allreduce(gpbdev_vecchia_t h, gpbdev_allreduce_fn fn, void* ctx);
 GPBDEV_EXPORT int gpbdev_fp64_peak(int device, double* tflops);
