@@ -213,3 +213,47 @@ def rows_ld(coords, nn_rows, cid, var, range_, diag_nb, diag_obs, y, row_begin=0
         C.c_double(COV_EVAL_ULPS), C.c_double(dist_ulps(d)), C.c_double(cov_mult), None if dr is None else _p(dr, C.c_int64),
         _p(out), _p(A), _p(bA))
     return {k: out[:, j] for j, k in enumerate(ROWS_COLS)}, A, bA, bad
+
+
+# ---- long-double per-row reference of the anisotropic gradient pass (orc_vecchia_rows_aniso_ld)
+ANISO_COLS = ["D", "By", "u", "quad", "logD", "bD", "bBy", "bu", "bquad", "blogD", "kappa", "eps"]
+
+
+def share_ulps(d, d_c):
+    """extra relative error, in units of u, of one group entry g S_c / r^2 of the device over the isotropic derivative g: the
+    division (1), S_c (d_c differences and their fused squares summed: d_c + 2), the r^2 it is divided by (d + 2) and the final
+    multiply (1)"""
+    return d + d_c + 6.
+
+
+def rows_aniso_ld(coords_scaled, nn_rows, cid, var, group_of_coord, y, row_begin=0, group_mult=None, swap=None, drop=None,
+                  unmasked=None):
+    """Rows [row_begin, row_begin + len(nn_rows)) of the anisotropic gradient pass in long double at range 1 on the scaled
+    coordinates (n, d) in Vecchia order, with first-order bounds of an fp64 evaluation (oracle/vecchia_oracle.c:
+    orc_vecchia_rows_aniso_ld). Deliberate faults: group_mult = (c, 1 + delta), swap = (row, c1, c2), drop = (row, c, a, b) (a, b:
+    points of the row, its neighbours in slot order then the row itself), unmasked = c. Returns (dict, bad): the columns of
+    ANISO_COLS, "terms" (nrows, 3 (1 + C)) in the order of the device's sums 3.. and "bterms" their bounds."""
+    coords = np.asarray(coords_scaled, dtype=np.float64)
+    n, d = coords.shape
+    nn_rows = np.ascontiguousarray(nn_rows, dtype=np.int32)
+    nrows, m = nn_rows.shape
+    grp = np.ascontiguousarray(group_of_coord, dtype=np.int32)
+    ng = int(grp.max()) + 1
+    np_ = 1 + ng
+    ulps = np.array([share_ulps(d, int(np.sum(grp == c))) for c in range(ng)])
+    out = np.empty((nrows, 12 + 6 * np_))
+    mg, mult = (-1, 1.) if group_mult is None else (int(group_mult[0]), float(group_mult[1]))
+    sw = None if swap is None else np.ascontiguousarray(swap, dtype=np.int64)
+    dr = None if drop is None else np.ascontiguousarray(drop, dtype=np.int64)
+    L = lib()
+    L.orc_vecchia_rows_aniso_ld.restype = C.c_int
+    bad = L.orc_vecchia_rows_aniso_ld(
+        _p(np.asfortranarray(coords)), C.c_int64(n), C.c_int(d), C.c_int(m), _p(nn_rows, C.c_int32), C.c_int(cid), C.c_double(var),
+        _p(grp, C.c_int32), C.c_int(ng), _p(np.ascontiguousarray(y, dtype=np.float64)), C.c_int64(row_begin), C.c_int64(nrows),
+        C.c_double(COV_EVAL_ULPS), C.c_double(dist_ulps(d)), _p(ulps), C.c_int(mg), C.c_double(mult),
+        None if sw is None else _p(sw, C.c_int64), None if dr is None else _p(dr, C.c_int64), C.c_int(-1 if unmasked is None else unmasked),
+        _p(out))
+    r = {k: out[:, j] for j, k in enumerate(ANISO_COLS)}
+    r["terms"] = out[:, 12:12 + 3 * np_]
+    r["bterms"] = out[:, 12 + 3 * np_:]
+    return r, bad

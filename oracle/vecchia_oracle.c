@@ -554,6 +554,90 @@ static void orc_chol_solve_ld(const orc_ld* l, int q, int ld, orc_ld* b) {
   }
 }
 
+/* One row after its augmented matrix is built: St (q + 1 points, both triangles and the diagonal) and the off-diagonal evaluation
+ * errors in E. Adds the diagonal and Cholesky terms of E, factors S_NN, solves a = S_NN^-1 s and w = S_NN^-1 y_N, forms S_NN^-1
+ * (Si), D, By and their bounds, and leaves b = [-a, 1] in a, wt = [w, 0] in w and E |b| in t. Returns -1 when S_NN is not
+ * positive definite. */
+typedef struct {
+  orc_ld D, By, uu, bD, bBy, bu, Mu, kap, eps;
+} orc_row_ld;
+
+static int orc_row_factor_ld(int q, int M, orc_ld u, const orc_ld* St, orc_ld* E, const orc_ld* yn, orc_ld* L, orc_ld* Si,
+                             orc_ld* a, orc_ld* w, orc_ld* t, orc_row_ld* rw) {
+  const orc_ld gam = (q + 2) * u / (1.L - (q + 2) * u);
+  orc_ld eps = 0.L;
+  for (int p = 0; p <= q; ++p) {
+    E[p * M + p] = u * fabsl(St[p * M + p]) + gam * St[p * M + p];
+    for (int s = 0; s < p; ++s) {
+      const orc_ld sc = sqrtl(St[p * M + p] * St[s * M + s]);
+      E[p * M + s] += gam * sc;
+      E[s * M + p] = E[p * M + s];
+    }
+    for (int s = 0; s <= p; ++s) eps = fmaxl(eps, E[p * M + s] / sqrtl(St[p * M + p] * St[s * M + s]));
+  }
+  for (int p = 0; p < q; ++p)
+    for (int s = 0; s < q; ++s) L[p * M + s] = St[p * M + s];
+  if (orc_chol_ld(L, q, M) != 0) return -1;
+  for (int p = 0; p < q; ++p) { a[p] = St[p * M + q]; w[p] = yn[p]; }
+  orc_chol_solve_ld(L, q, M, a);
+  orc_chol_solve_ld(L, q, M, w);
+  for (int c = 0; c < q; ++c) { /* S_NN^-1, column c */
+    for (int p = 0; p < q; ++p) t[p] = p == c ? 1.L : 0.L;
+    orc_chol_solve_ld(L, q, M, t);
+    for (int p = 0; p < q; ++p) Si[p * M + c] = t[p];
+  }
+  orc_ld D = St[q * M + q], By = yn[q];
+  for (int p = 0; p < q; ++p) { D -= a[p] * St[p * M + q]; By -= a[p] * yn[p]; }
+  /* b = [-a, 1], wt = [w, 0] */
+  a[q] = -1.L; w[q] = 0.L;
+  orc_ld bD = 0.L, bBy = 0.L, ay = fabsl(yn[q]);
+  for (int p = 0; p <= q; ++p) {
+    orc_ld eb = 0.L;
+    for (int s = 0; s <= q; ++s) eb += E[p * M + s] * fabsl(a[s]);
+    bD += fabsl(a[p]) * eb;
+    bBy += fabsl(w[p]) * eb;
+    t[p] = eb;
+    if (p < q) ay += fabsl(a[p] * yn[p]);
+  }
+  bBy += gam * ay;
+  orc_ld n1 = 0.L, ni = 0.L; /* kappa_1 = |S|_1 |S^-1|_1 */
+  for (int c = 0; c < q; ++c) {
+    orc_ld s1 = 0.L, s2 = 0.L;
+    for (int p = 0; p < q; ++p) { s1 += fabsl(St[p * M + c]); s2 += fabsl(Si[p * M + c]); }
+    n1 = fmaxl(n1, s1); ni = fmaxl(ni, s2);
+  }
+  rw->D = D; rw->By = By; rw->uu = By / D; rw->bD = bD; rw->bBy = bBy;
+  rw->bu = bBy / D + fabsl(By) * bD / (D * D);
+  rw->Mu = ay / D;
+  rw->kap = q > 0 ? n1 * ni : 1.L;
+  rw->eps = eps;
+  return 0;
+}
+
+/* The three GRAD accumulator terms of one parameter with derivative matrix G (u_k u, u^2 dD_k, dD_k / D; u_k = -(g - G_NN A).w,
+ * dD_k = G_qq - 2 A.g + A^T G_NN A, g = G_Nq) and their bounds ke (magnitude of the term with every factor in absolute value):
+ * o[0..2] the terms, o[3..5] the bounds. a, w as orc_row_factor_ld leaves them. */
+static void orc_row_grad_ld(const orc_ld* G, int q, int M, const orc_ld* a, const orc_ld* w, const orc_row_ld* rw, orc_ld ke,
+                            orc_ld* o) {
+  orc_ld uk = 0.L, Muk = 0.L, dD = G[q * M + q], MdD = fabsl(G[q * M + q]);
+  for (int p = 0; p < q; ++p) {
+    orc_ld ga = 0.L, gaa = 0.L;
+    for (int s = 0; s < q; ++s) { ga += G[p * M + s] * a[s]; gaa += fabsl(G[p * M + s] * a[s]); }
+    const orc_ld g = G[p * M + q];
+    uk -= (g - ga) * w[p];
+    Muk += (fabsl(g) + gaa) * fabsl(w[p]);
+    dD += -2.L * a[p] * g + a[p] * ga;
+    MdD += 2.L * fabsl(a[p] * g) + fabsl(a[p]) * gaa;
+  }
+  const orc_ld uu = rw->uu, Mu = rw->Mu, D = rw->D;
+  o[0] = uk * uu;
+  o[1] = uu * uu * dD;
+  o[2] = dD / D;
+  o[3] = ke * (Muk * fabsl(uu) + fabsl(uk) * Mu);
+  o[4] = ke * (uu * uu * MdD + 2.L * fabsl(uu) * Mu * fabsl(dD));
+  o[5] = ke * (MdD + fabsl(dD)) / D;
+}
+
 int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int32_t* nn, int cov_type, double var_d,
                         double range_d, double diag_nb, double diag_obs, const double* y, const double* qcoords, int64_t row_begin,
                         int64_t nrows, double cv, double cr, double cov_mult, const int64_t* drop, double* out, double* A,
@@ -595,7 +679,6 @@ int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int
         xn[j] = mx;
         yn[j] = j < q ? (orc_ld)y[nb[pos[j]]] : (qcoords ? 0.L : (orc_ld)y[i]);
       }
-      const orc_ld gam = (q + 2) * u / (1.L - (q + 2) * u);
       orc_ld rho = 0.L; /* largest relative evaluation error of one covariance */
       for (int p = 0; p <= q; ++p) {
         St[p * M + p] = p < q ? (orc_ld)diag_nb : (orc_ld)diag_obs;
@@ -617,83 +700,166 @@ int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int
           if (c0 != 0.L) rho = fmaxl(rho, E[p * M + s] / fabsl(c0));
         }
       }
-      orc_ld eps = 0.L;
-      for (int p = 0; p <= q; ++p) {
-        E[p * M + p] = u * fabsl(St[p * M + p]) + gam * St[p * M + p];
-        for (int s = 0; s < p; ++s) {
-          const orc_ld sc = sqrtl(St[p * M + p] * St[s * M + s]);
-          E[p * M + s] += gam * sc;
-          E[s * M + p] = E[p * M + s];
-        }
-        for (int s = 0; s <= p; ++s) eps = fmaxl(eps, E[p * M + s] / sqrtl(St[p * M + p] * St[s * M + s]));
+      orc_row_ld rw;
+      if (orc_row_factor_ld(q, M, u, St, E, yn, L, Si, a, w, t, &rw) != 0) {
+        ++bad;
+        for (int k = 0; k < ORC_ROWS_NOUT; ++k) o[k] = NAN;
+        continue;
       }
-      for (int p = 0; p < q; ++p)
-        for (int s = 0; s < q; ++s) L[p * M + s] = St[p * M + s];
-      if (orc_chol_ld(L, q, M) != 0) { ++bad; for (int k = 0; k < ORC_ROWS_NOUT; ++k) o[k] = NAN; continue; }
-      for (int p = 0; p < q; ++p) { a[p] = St[p * M + q]; w[p] = yn[p]; }
-      orc_chol_solve_ld(L, q, M, a);
-      orc_chol_solve_ld(L, q, M, w);
-      for (int c = 0; c < q; ++c) { /* S_NN^-1, column c */
-        for (int p = 0; p < q; ++p) t[p] = p == c ? 1.L : 0.L;
-        orc_chol_solve_ld(L, q, M, t);
-        for (int p = 0; p < q; ++p) Si[p * M + c] = t[p];
-      }
-      orc_ld D = St[q * M + q], By = yn[q];
-      for (int p = 0; p < q; ++p) { D -= a[p] * St[p * M + q]; By -= a[p] * yn[p]; }
+      const orc_ld D = rw.D, By = rw.By;
       if (!(D > 0.L)) ++bad;
-      const orc_ld uu = By / D;
-      /* b = [-a, 1], wt = [w, 0] */
-      a[q] = -1.L; w[q] = 0.L;
-      orc_ld bD = 0.L, bBy = 0.L, ay = fabsl(yn[q]);
-      for (int p = 0; p <= q; ++p) {
-        orc_ld eb = 0.L;
-        for (int s = 0; s <= q; ++s) eb += E[p * M + s] * fabsl(a[s]);
-        bD += fabsl(a[p]) * eb;
-        bBy += fabsl(w[p]) * eb;
-        t[p] = eb;
-        if (p < q) ay += fabsl(a[p] * yn[p]);
-      }
-      bBy += gam * ay;
       for (int p = 0; p < q; ++p) {
         orc_ld s = 0.L;
         for (int c = 0; c < q; ++c) s += fabsl(Si[p * M + c]) * t[c];
         A[(size_t)r * m + pos[p]] = (double)a[p];
         bA[(size_t)r * m + pos[p]] = (double)s;
       }
-      orc_ld n1 = 0.L, ni = 0.L; /* kappa_1 = |S|_1 |S^-1|_1 */
-      for (int c = 0; c < q; ++c) {
-        orc_ld s1 = 0.L, s2 = 0.L;
-        for (int p = 0; p < q; ++p) { s1 += fabsl(St[p * M + c]); s2 += fabsl(Si[p * M + c]); }
-        n1 = fmaxl(n1, s1); ni = fmaxl(ni, s2);
-      }
-      const orc_ld kap = q > 0 ? n1 * ni : 1.L, ke = kap * (eps + rho);
-      const orc_ld bu = bBy / D + fabsl(By) * bD / (D * D), Mu = ay / D;
-      o[0] = (double)D; o[1] = (double)By; o[2] = (double)uu; o[3] = (double)(By * By / D); o[4] = (double)logl(D);
-      o[11] = (double)bD; o[12] = (double)bBy; o[13] = (double)bu;
+      const orc_ld ke = rw.kap * (rw.eps + rho), bD = rw.bD, bBy = rw.bBy;
+      o[0] = (double)D; o[1] = (double)By; o[2] = (double)rw.uu; o[3] = (double)(By * By / D); o[4] = (double)logl(D);
+      o[11] = (double)bD; o[12] = (double)bBy; o[13] = (double)rw.bu;
       o[14] = (double)(2.L * fabsl(By) * bBy / D + By * By * bD / (D * D) + 3.L * u * By * By / D);
       o[15] = (double)(bD / D + u * (1.L + fabsl(logl(D))));
-      o[22] = (double)kap; o[23] = (double)eps;
-      for (int k = 0; k < 2; ++k) { /* u_k = -(g - G_NN A).(S_NN^-1 y_N), dD_k = G_qq - 2 A.g + A^T G_NN A (g = G_Nq) */
-        const orc_ld* G = k == 0 ? G0 : G1;
-        orc_ld uk = 0.L, Muk = 0.L, dD = G[q * M + q], MdD = fabsl(G[q * M + q]);
-        for (int p = 0; p < q; ++p) {
-          orc_ld ga = 0.L, gaa = 0.L;
-          for (int s = 0; s < q; ++s) { ga += G[p * M + s] * a[s]; gaa += fabsl(G[p * M + s] * a[s]); }
-          const orc_ld g = G[p * M + q];
-          uk -= (g - ga) * w[p];
-          Muk += (fabsl(g) + gaa) * fabsl(w[p]);
-          dD += -2.L * a[p] * g + a[p] * ga;
-          MdD += 2.L * fabsl(a[p] * g) + fabsl(a[p]) * gaa;
-        }
-        o[5 + k] = (double)(uk * uu);
-        o[7 + k] = (double)(uu * uu * dD);
-        o[9 + k] = (double)(dD / D);
-        o[16 + k] = (double)(ke * (Muk * fabsl(uu) + fabsl(uk) * Mu));
-        o[18 + k] = (double)(ke * (uu * uu * MdD + 2.L * fabsl(uu) * Mu * fabsl(dD)));
-        o[20 + k] = (double)(ke * (MdD + fabsl(dD)) / D);
+      o[22] = (double)rw.kap; o[23] = (double)rw.eps;
+      for (int k = 0; k < 2; ++k) {
+        orc_ld g6[6];
+        orc_row_grad_ld(k == 0 ? G0 : G1, q, M, a, w, &rw, ke, g6);
+        o[5 + k] = (double)g6[0]; o[7 + k] = (double)g6[1]; o[9 + k] = (double)g6[2];
+        o[16 + k] = (double)g6[3]; o[18 + k] = (double)g6[4]; o[20 + k] = (double)g6[5];
       }
     }
     free(x); free(xn); free(St); free(E); free(G0); free(G1); free(L); free(Si); free(a); free(w); free(yn); free(t); free(pos);
+  }
+  return bad;
+}
+
+/* ---- long-double reference of the anisotropic gradient pass (MODE_GRAD_ANISO / BIG_GRAD_ANISO), rows [row_begin, row_begin + nrows)
+ *
+ * coords are the SCALED coordinates (n x d column-major, Vecchia order); the kernel is the isotropic closed form at range 1 on them,
+ * diagonal var + 1 for neighbours and the row's own point. group_of_coord (d entries) assigns every coordinate to one of ngroups
+ * groups. D, By, their bounds, kappa and eps are those of orc_vecchia_rows_ld at range 1. For k = 0 (log var: dSigma = Sigma
+ * without the nugget) and k = 1..ngroups (log lambda of group c = k - 1) the three GRAD terms u_k u, u^2 dD_k, dD_k / D come from
+ * each parameter's derivative matrix, whose off-diagonal entries are the element formulas of the kernels on the scaled
+ * differences, with S_c = sum of the squared differences over the coordinates of group c and r^2 = sum over all coordinates:
+ *   exponential  -var e^-r S_c / r      Matern 1.5  -var e^-r S_c      Matern 2.5  -var (1 + r) / 3 e^-r S_c      Gaussian  -var e^-r^2 S_c
+ * (0 at r = 0; the diagonal is 0). Bounds: kappa (eps + rho) times the term's magnitude for k = 0, as orc_vecchia_rows_ld; the
+ * group terms add to rho the roundings of the device's split g S_c / r^2 of one entry: share_ulps[c] u (the caller's count of the
+ * division, the roundings of S_c and of r^2, and the final multiply).
+ *
+ * out: nrows x (12 + 6 (1 + ngroups)), columns
+ *   0 D  1 By  2 u  3 By^2 / D  4 log D  5 beta_D  6 beta_By  7 beta_u  8 beta(By^2 / D)  9 beta(log D)  10 kappa  11 eps
+ *   12 + 3 k + j: term j of parameter k (j = 0 u_k u, 1 u^2 dD_k, 2 dD_k / D)    12 + 3 (1 + ngroups) + 3 k + j: its bound
+ * Deliberate faults, for tests of the bounds themselves: every entry of group mult_group scaled by mult (mult_group -1: none);
+ * swap = {row, c1, c2}: groups c1 and c2 exchange their matrices in one row; drop = {row, c, a, b}: the pair (a, b) is missing
+ * from group c's matrix in one row; unmasked = c: group c uses r^2 instead of S_c (-1: none).
+ * Returns the number of rows whose neighbour block is not positive definite. */
+static orc_ld orc_aniso_share_ld(int type, orc_ld dist, orc_ld var) {
+  if (dist == 0.L) return 0.L;
+  switch (type) {
+    case ORC_COV_EXPONENTIAL: return -var * expl(-dist) / dist;
+    case ORC_COV_MATERN15: return -var * expl(-dist);
+    case ORC_COV_MATERN25: return -var * (1.L + dist) / 3.L * expl(-dist);
+    default: return -var * expl(-dist * dist);
+  }
+}
+
+int orc_vecchia_rows_aniso_ld(const double* coords, int64_t n, int d, int m, const int32_t* nn, int cov_type, double var_d,
+                              const int32_t* group_of_coord, int ngroups, const double* y, int64_t row_begin, int64_t nrows,
+                              double cv, double cr, const double* share_ulps, int mult_group, double mult, const int64_t* swap,
+                              const int64_t* drop, int unmasked, double* out) {
+  const orc_ld u = ldexpl(1.L, -53), var = var_d, diag = var + 1.L;
+  const int M = m + 1, NP = 1 + ngroups, nout = 12 + 6 * NP;
+  int bad = 0;
+#pragma omp parallel
+  {
+    orc_ld* x = (orc_ld*)malloc(sizeof(orc_ld) * M * d);
+    orc_ld* xn = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* St = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* E = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* G = (orc_ld*)malloc(sizeof(orc_ld) * NP * M * M);  /* parameter k: G + k M M */
+    orc_ld* L = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* Si = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* a = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* w = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* yn = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* t = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* Sc = (orc_ld*)malloc(sizeof(orc_ld) * ngroups);
+    int* pos = (int*)malloc(sizeof(int) * M);
+#pragma omp for schedule(dynamic, 64) reduction(+ : bad)
+    for (int64_t r = 0; r < nrows; ++r) {
+      const int64_t i = row_begin + r;
+      const int32_t* nb = nn + (size_t)r * m;
+      double* o = out + (size_t)r * nout;
+      int q = 0;
+      for (int k = 0; k < m; ++k)
+        if (nb[k] >= 0) pos[q++] = k;
+      for (int c = 0; c < d; ++c) {
+        for (int j = 0; j < q; ++j) x[j * d + c] = coords[(size_t)c * n + nb[pos[j]]];
+        x[q * d + c] = coords[(size_t)c * n + i];
+      }
+      for (int j = 0; j <= q; ++j) {
+        orc_ld mx = 0.L;
+        for (int c = 0; c < d; ++c) mx = fmaxl(mx, fabsl(x[j * d + c]));
+        xn[j] = mx;
+        yn[j] = j < q ? (orc_ld)y[nb[pos[j]]] : (orc_ld)y[i];
+      }
+      orc_ld rho = 0.L;
+      for (int p = 0; p <= q; ++p) {
+        St[p * M + p] = diag;
+        G[p * M + p] = var;
+        for (int k = 1; k < NP; ++k) G[(size_t)k * M * M + p * M + p] = 0.L;
+        for (int s = p + 1; s <= q; ++s) {
+          orc_ld r2 = 0.L;
+          for (int c = 0; c < ngroups; ++c) Sc[c] = 0.L;
+          for (int c = 0; c < d; ++c) {
+            const orc_ld df = x[p * d + c] - x[s * d + c];
+            r2 += df * df;
+            Sc[group_of_coord[c]] += df * df;
+          }
+          const orc_ld dist = sqrtl(r2);
+          const orc_ld c0 = orc_cov_ld(cov_type, dist, var, 1.L);
+          const orc_ld dd = orc_cov_ddist_ld(cov_type, dist, var, 1.L);
+          const orc_ld sh = orc_aniso_share_ld(cov_type, dist, var);
+          St[p * M + s] = St[s * M + p] = c0;
+          G[p * M + s] = G[s * M + p] = c0;
+          for (int c = 0; c < ngroups; ++c) {
+            orc_ld g = sh * (c == unmasked ? r2 : Sc[c]);
+            if (c == mult_group) g *= mult;
+            if (drop && drop[0] == r && drop[1] == c && ((drop[2] == p && drop[3] == s) || (drop[2] == s && drop[3] == p))) g = 0.L;
+            G[(size_t)(1 + c) * M * M + p * M + s] = G[(size_t)(1 + c) * M * M + s * M + p] = g;
+          }
+          E[p * M + s] = E[s * M + p] = u * (cv * fabsl(c0) + fabsl(dd) * (cr * dist + sqrtl((orc_ld)d) * (xn[p] + xn[s])));
+          if (c0 != 0.L) rho = fmaxl(rho, E[p * M + s] / fabsl(c0));
+        }
+      }
+      if (swap && swap[0] == r) {
+        orc_ld* g1 = G + (size_t)(1 + swap[1]) * M * M;
+        orc_ld* g2 = G + (size_t)(1 + swap[2]) * M * M;
+        for (int e = 0; e < M * M; ++e) { const orc_ld tmp = g1[e]; g1[e] = g2[e]; g2[e] = tmp; }
+      }
+      orc_row_ld rw;
+      if (orc_row_factor_ld(q, M, u, St, E, yn, L, Si, a, w, t, &rw) != 0) {
+        ++bad;
+        for (int k = 0; k < nout; ++k) o[k] = NAN;
+        continue;
+      }
+      const orc_ld D = rw.D, By = rw.By, bD = rw.bD, bBy = rw.bBy;
+      if (!(D > 0.L)) ++bad;
+      o[0] = (double)D; o[1] = (double)By; o[2] = (double)rw.uu; o[3] = (double)(By * By / D); o[4] = (double)logl(D);
+      o[5] = (double)bD; o[6] = (double)bBy; o[7] = (double)rw.bu;
+      o[8] = (double)(2.L * fabsl(By) * bBy / D + By * By * bD / (D * D) + 3.L * u * By * By / D);
+      o[9] = (double)(bD / D + u * (1.L + fabsl(logl(D))));
+      o[10] = (double)rw.kap; o[11] = (double)rw.eps;
+      for (int k = 0; k < NP; ++k) {
+        orc_ld g6[6];
+        const orc_ld rk = k == 0 ? rho : rho + (orc_ld)share_ulps[k - 1] * u;
+        orc_row_grad_ld(G + (size_t)k * M * M, q, M, a, w, &rw, rw.kap * (rw.eps + rk), g6);
+        for (int j = 0; j < 3; ++j) {
+          o[12 + 3 * k + j] = (double)g6[j];
+          o[12 + 3 * NP + 3 * k + j] = (double)g6[3 + j];
+        }
+      }
+    }
+    free(x); free(xn); free(St); free(E); free(G); free(L); free(Si); free(a); free(w); free(yn); free(t); free(Sc); free(pos);
   }
   return bad;
 }

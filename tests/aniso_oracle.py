@@ -107,6 +107,15 @@ class AnisoOracle:
 
     def grad_profiled(self, cov_pars, y):
         """(negll, gradient w.r.t. log(var ratio), log(lambda_1..C)) with the error variance profiled out, at the current sets"""
+        quad, logdet, uk, udu, tr = self.grad_sums(cov_pars, y)
+        n = self.n
+        s2 = quad / n
+        negll = quad / 2. / s2 + logdet / 2. + n / 2. * (np.log(s2) + np.log(2 * np.pi))
+        return negll, (uk - 0.5 * udu) / s2 + 0.5 * tr
+
+    def grad_sums(self, cov_pars, y):
+        """the sums of the device's gradient pass at the current sets: sum (By)^2 / D, sum log D and, per parameter (log var ratio,
+        log lambda_1..C), sum u_k u, sum u^2 dD_k and sum dD_k / D"""
         _, var, lam = transform(cov_pars, self.cov_function, self.shape)
         yo = np.asarray(y, dtype=np.float64)[self.perm]
         C = lam.shape[0]
@@ -138,9 +147,7 @@ class AnisoOracle:
                 uk[kk] += dBy * u
                 udu[kk] += u * u * dD
                 tr[kk] += dD / D
-        s2 = quad / n
-        negll = quad / 2. / s2 + logdet / 2. + n / 2. * (np.log(s2) + np.log(2 * np.pi))
-        return negll, (uk - 0.5 * udu) / s2 + 0.5 * tr
+        return quad, logdet, uk, udu, tr
 
 
 def init_cov_pars(coords_ordered, y, cov_function, shape):
