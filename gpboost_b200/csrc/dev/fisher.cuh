@@ -117,18 +117,46 @@ int fisher_factor(gpbdev_vecchia* h, int cov_type, double var, double range, Fis
   return 0;
 }
 
+// what the Fisher information and the read-back of its factor refuse besides null buffers and the probe block
+int fisher_refuse(const gpbdev_vecchia* h, int cov_type, double var, double range, const std::string& fn) {
+  if (cov_type < 0 || cov_type > 3) return fail(fn + ": unknown covariance id");
+  if (!(var > 0.) || !(range > 0.)) return fail(fn + ": covariance parameters must be positive");
+  if (h->row_begin != 0 || h->row_end != h->n) return fail(fn + ": row-sharded engines are not supported");
+  if (h->m > gpl::kM) return fail(fn + ": num_neighbors must be <= 30");
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
 
+int gpbdev_vecchia_gaussian_factor_grad(gpbdev_vecchia_t h, int cov_type, double var, double range, double* A_host, double* Dinv_host,
+                                        double* dA0_host, double* dD0_host, double* dA1_host, double* dD1_host) {
+  if (!h || !A_host || !Dinv_host || !dA0_host || !dD0_host || !dA1_host || !dD1_host)
+    return fail("gpbdev_vecchia_gaussian_factor_grad: null argument");
+  if (fisher_refuse(h, cov_type, var, range, "gpbdev_vecchia_gaussian_factor_grad")) return -1;
+  CUDA_TRY(cudaSetDevice(h->device));
+  const size_t nb = sizeof(double) * (size_t)h->n, nbm = nb * h->m;
+  FisherBufs f;
+  CUDA_TRY(cudaMalloc(&f.A, nbm)); CUDA_TRY(cudaMalloc(&f.dA0, nbm)); CUDA_TRY(cudaMalloc(&f.dA1, nbm));
+  CUDA_TRY(cudaMalloc(&f.Dinv, nb)); CUDA_TRY(cudaMalloc(&f.w, nb)); CUDA_TRY(cudaMalloc(&f.dD0, nb)); CUDA_TRY(cudaMalloc(&f.dD1, nb));
+  if (fisher_factor(h, cov_type, var, range, f)) return -1;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  CUDA_TRY(cudaMemcpy(A_host, f.A, nbm, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(Dinv_host, f.Dinv, nb, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(dA0_host, f.dA0, nbm, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(dD0_host, f.dD0, nb, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(dA1_host, f.dA1, nbm, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(dD1_host, f.dD1, nb, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int gpbdev_vecchia_fisher_info(gpbdev_vecchia_t h, int cov_type, double sigma2, double var, double range, const double* probes_colmajor,
                                int t, double* FI9) {
   if (!h || !probes_colmajor || !FI9) return fail("gpbdev_vecchia_fisher_info: null argument");
-  if (cov_type < 0 || cov_type > 3) return fail("gpbdev_vecchia_fisher_info: unknown covariance id");
-  if (!(sigma2 > 0.) || !(var > 0.) || !(range > 0.)) return fail("gpbdev_vecchia_fisher_info: covariance parameters must be positive");
+  if (!(sigma2 > 0.)) return fail("gpbdev_vecchia_fisher_info: covariance parameters must be positive");
   if (t < 1) return fail("gpbdev_vecchia_fisher_info: need at least one probe vector");
-  if (h->row_begin != 0 || h->row_end != h->n) return fail("gpbdev_vecchia_fisher_info: row-sharded engines are not supported");
-  if (h->m > gpl::kM) return fail("gpbdev_vecchia_fisher_info: num_neighbors must be <= 30");
+  if (fisher_refuse(h, cov_type, var, range, "gpbdev_vecchia_fisher_info")) return -1;
   CUDA_TRY(cudaSetDevice(h->device));
   if (laplace_ensure(h)) return -1;
   if (ensure_csc(h)) return -1;

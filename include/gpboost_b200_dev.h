@@ -181,6 +181,14 @@ GPBDEV_EXPORT int gpbdev_vecchia_latent_factor_grad(gpbdev_vecchia_t h, int cov_
  * its last sums and its STORE shortcut state are not touched. */
 GPBDEV_EXPORT int gpbdev_vecchia_fisher_info(gpbdev_vecchia_t h, int cov_type, double sigma2, double var, double range,
                                              const double* probes_colmajor, int t, double* FI9);
+/* The Gaussian factor (nugget 1 on the transformed scale) with its derivatives w.r.t. log(var) and log(range) — B_grad[0..1] = -dA,
+ * D_grad[0..1] = dD of CalcCovFactorGradientVecchia (src/GPBoost/Vecchia_utils.cpp:1636-1652) — as gpbdev_vecchia_fisher_info forms
+ * them (the factor kernel's MODE_STORE_GRAD2, launched by the same routine), copied to host buffers (A, dA0, dA1: n x m row-major in
+ * Vecchia order; Dinv, dD0, dD1: n). Refuses what gpbdev_vecchia_fisher_info refuses; leaves the engine's stored factor, its last
+ * sums and its STORE shortcut state alone. Diagnostics / test entry. */
+GPBDEV_EXPORT int gpbdev_vecchia_gaussian_factor_grad(gpbdev_vecchia_t h, int cov_type, double var, double range, double* A_host,
+                                                      double* Dinv_host, double* dA0_host, double* dD0_host, double* dA1_host,
+                                                      double* dD1_host);
 /* After a STORE eval: copy A (n x m) and D^-1 (n) to the host — parity tests against the oracle's B, D^-1 */
 GPBDEV_EXPORT int gpbdev_vecchia_get_factor(gpbdev_vecchia_t h, double* A_host, double* Dinv_host);
 

@@ -6,6 +6,8 @@ High-level entry points mirror what the reference's C API computes for the hot p
   * `nll_and_grad(...)`        ==  one EvalLLforLBFGSpp objective + gradient call (optim_utils.h:244-340)
 """
 import ctypes as C
+import math
+
 import numpy as np
 
 from .build import build_oracle
@@ -257,3 +259,36 @@ def rows_aniso_ld(coords_scaled, nn_rows, cid, var, group_of_coord, y, row_begin
     r["terms"] = out[:, 12:12 + 3 * np_]
     r["bterms"] = out[:, 12 + 3 * np_:]
     return r, bad
+
+
+# ---- long-double per-row reference of the factor derivatives (orc_vecchia_rows_dfactor_ld)
+DF_COLS = ["D", "bD", "dD0", "bdD0", "dD1", "bdD1", "kappa", "eps", "rho0", "rho1"]
+# relative error of one fp64 evaluation of the range derivative's closed form in units of u: the covariance's (COV_EVAL_ULPS) and
+# up to four more products (range, distance and variance factors)
+GRAD_EVAL_ULPS = COV_EVAL_ULPS + 4.
+# the kernels' exp(-x) saturates at exp(-700) (vecchia_factor.cuh: exp_neg): the absolute error of exp(-x) for x > 700
+EXP_FLOOR = math.exp(-700.)
+
+
+def rows_dfactor_ld(coords, nn_rows, cid, var, range_, diag_nb, diag_obs, row_begin=0, range_mult=1.0, drop=None, g1_diag=0.0,
+                    g0_shift=0.0):
+    """Rows [row_begin, row_begin + len(nn_rows)) of the factor derivatives w.r.t. log var (k = 0) and log range (k = 1) in long
+    double, dA_k = S_NN^-1 (g_k - G_k,NN A) and dD_k = b^T G_k b, with first-order bounds of an fp64 evaluation whose exp(-x) may
+    saturate at EXP_FLOOR (oracle/vecchia_oracle.c: orc_vecchia_rows_dfactor_ld). diag_nb / diag_obs as rows_ld: var + 1 twice for the Gaussian factor,
+    var (1 + 1e-10) and var for the latent one. Deliberate faults: range_mult scales the range derivative, drop = (row, a, b) removes
+    one pair from it, g1_diag puts a value on its neighbour diagonal, g0_shift moves the variance derivative's diagonal. Returns
+    (dict of DF_COLS -> (nrows,), dA (2, nrows, m), bound of dA (2, nrows, m), number of bad rows)."""
+    coords = np.asarray(coords, dtype=np.float64)
+    n, d = coords.shape
+    nn_rows = np.ascontiguousarray(nn_rows, dtype=np.int32)
+    nrows, m = nn_rows.shape
+    out = np.empty((nrows, len(DF_COLS))); dA = np.empty((2, nrows, m)); bdA = np.empty((2, nrows, m))
+    dr = None if drop is None else np.ascontiguousarray(drop, dtype=np.int64)
+    L = lib()
+    L.orc_vecchia_rows_dfactor_ld.restype = C.c_int
+    bad = L.orc_vecchia_rows_dfactor_ld(
+        _p(np.asfortranarray(coords)), C.c_int64(n), C.c_int(d), C.c_int(m), _p(nn_rows, C.c_int32), C.c_int(cid), C.c_double(var),
+        C.c_double(range_), C.c_double(diag_nb), C.c_double(diag_obs), C.c_int64(row_begin), C.c_int64(nrows),
+        C.c_double(COV_EVAL_ULPS), C.c_double(dist_ulps(d)), C.c_double(GRAD_EVAL_ULPS), C.c_double(EXP_FLOOR), C.c_double(range_mult),
+        None if dr is None else _p(dr, C.c_int64), C.c_double(g1_diag), C.c_double(g0_shift), _p(out), _p(dA), _p(bdA))
+    return {k: out[:, j] for j, k in enumerate(DF_COLS)}, dA, bdA, bad

@@ -526,6 +526,29 @@ static orc_ld orc_cov_grad_range_ld(int type, orc_ld dist, orc_ld var, orc_ld ra
   return type == ORC_COV_GAUSSIAN ? 0.5L * g : g;
 }
 
+/* exponent x of the covariance's exp(-x) and the factors multiplying exp(-x) in the covariance (pre[0]) and in its log-range
+ * derivative (pre[1]) */
+static orc_ld orc_exp_arg_ld(int type, orc_ld dist, orc_ld var, orc_ld range, orc_ld* pre) {
+  const orc_ld rd = range * dist;
+  switch (type) {
+    case ORC_COV_EXPONENTIAL: pre[0] = var; pre[1] = rd * var; return rd;
+    case ORC_COV_MATERN15: pre[0] = var * (1.L + rd); pre[1] = var * rd * rd; return rd;
+    case ORC_COV_MATERN25: pre[0] = var * (1.L + rd + rd * rd / 3.L); pre[1] = var * rd * rd * (1.L + rd) / 3.L; return rd;
+    default: pre[0] = var; pre[1] = rd * dist * var; return rd * dist;
+  }
+}
+
+/* d/d dist of orc_cov_grad_range_ld */
+static orc_ld orc_cov_grad_range_ddist_ld(int type, orc_ld dist, orc_ld var, orc_ld range) {
+  const orc_ld rd = range * dist;
+  switch (type) {
+    case ORC_COV_EXPONENTIAL: return -range * var * (1.L - rd) * expl(-rd);
+    case ORC_COV_MATERN15: return -var * range * range * dist * (2.L - rd) * expl(-rd);
+    case ORC_COV_MATERN25: return -var * range * range / 3.L * dist * (2.L + 2.L * rd - rd * rd) * expl(-rd);
+    default: return -2.L * range * var * dist * (1.L - range * dist * dist) * expl(-range * dist * dist);
+  }
+}
+
 static int orc_chol_ld(orc_ld* a, int q, int ld) {
   for (int j = 0; j < q; ++j) {
     orc_ld s = a[j * ld + j];
@@ -616,7 +639,7 @@ static int orc_row_factor_ld(int q, int M, orc_ld u, const orc_ld* St, orc_ld* E
 
 /* The three GRAD accumulator terms of one parameter with derivative matrix G (u_k u, u^2 dD_k, dD_k / D; u_k = -(g - G_NN A).w,
  * dD_k = G_qq - 2 A.g + A^T G_NN A, g = G_Nq) and their bounds ke (magnitude of the term with every factor in absolute value):
- * o[0..2] the terms, o[3..5] the bounds. a, w as orc_row_factor_ld leaves them. */
+ * o[0..2] the terms, o[3..5] the bounds, o[6] dD_k and o[7] its magnitude. a, w as orc_row_factor_ld leaves them. */
 static void orc_row_grad_ld(const orc_ld* G, int q, int M, const orc_ld* a, const orc_ld* w, const orc_row_ld* rw, orc_ld ke,
                             orc_ld* o) {
   orc_ld uk = 0.L, Muk = 0.L, dD = G[q * M + q], MdD = fabsl(G[q * M + q]);
@@ -636,6 +659,75 @@ static void orc_row_grad_ld(const orc_ld* G, int q, int M, const orc_ld* a, cons
   o[3] = ke * (Muk * fabsl(uu) + fabsl(uk) * Mu);
   o[4] = ke * (uu * uu * MdD + 2.L * fabsl(uu) * Mu * fabsl(dD));
   o[5] = ke * (MdD + fabsl(dD)) / D;
+  o[6] = dD;
+  o[7] = MdD;
+}
+
+/* Row r of orc_vecchia_rows_ld / orc_vecchia_rows_dfactor_ld: gathers its points (neighbours in slot order into x[0..q), the own
+ * point into x[q]; -1 slots skipped, their slot numbers in pos) and their |x|_inf, the responses yn (0 without y), and builds the
+ * augmented matrix St (diagonal diag_nb / diag_obs, covariances scaled by mult, the pair drop = {row, a, b} zeroed), E's off-diagonal
+ * evaluation errors, G0 (Sigma~ - I: diagonal var) and G1 (d Sigma / d log range: diagonal 0) from the unfaulted covariances. *rho:
+ * the largest E_ab / |St_ab|. When F1 is given it receives the evaluation errors of G1's entries,
+ * u (cg |G1_ab| + |dG1/dr|_ab (cr r_ab + sqrt(d) (|x_a|_inf + |x_b|_inf))), 0 on the diagonal, and *rho1_out the largest
+ * F1_ab / |G1_ab|. efloor > 0: where the exponent x of a pair's exp(-x) exceeds 700, E_ab and F1_ab also take efloor times the
+ * factor multiplying exp(-x) (not counted in rho and rho1): an fp64 exp(-x) may saturate at efloor there. Returns q. */
+static int orc_row_build_ld(const double* coords, int64_t n, int d, int m, const int32_t* nb, int cov_type, orc_ld var, orc_ld range,
+                            double diag_nb, double diag_obs, const double* y, const double* qcoords, int64_t i, int64_t r, int64_t nrows,
+                            orc_ld cv, orc_ld cr, orc_ld mult, const int64_t* drop, orc_ld cg, int* pos, orc_ld* x, orc_ld* xn, orc_ld* yn,
+                            orc_ld* St, orc_ld* E, orc_ld* G0, orc_ld* G1, orc_ld* F1, orc_ld efloor, orc_ld* rho_out,
+                            orc_ld* rho1_out) {
+  const orc_ld u = ldexpl(1.L, -53);
+  const int M = m + 1;
+  int q = 0;
+  for (int k = 0; k < m; ++k)
+    if (nb[k] >= 0) pos[q++] = k;
+  for (int c = 0; c < d; ++c) {
+    for (int j = 0; j < q; ++j) x[j * d + c] = coords[(size_t)c * n + nb[pos[j]]];
+    x[q * d + c] = qcoords ? qcoords[(size_t)c * nrows + r] : coords[(size_t)c * n + i];
+  }
+  for (int j = 0; j <= q; ++j) {
+    orc_ld mx = 0.L;
+    for (int c = 0; c < d; ++c) mx = fmaxl(mx, fabsl(x[j * d + c]));
+    xn[j] = mx;
+    yn[j] = !y ? 0.L : (j < q ? (orc_ld)y[nb[pos[j]]] : (qcoords ? 0.L : (orc_ld)y[i]));
+  }
+  orc_ld rho = 0.L, rho1 = 0.L;
+  for (int p = 0; p <= q; ++p) {
+    St[p * M + p] = p < q ? (orc_ld)diag_nb : (orc_ld)diag_obs;
+    G0[p * M + p] = var;
+    G1[p * M + p] = 0.L;
+    if (F1) F1[p * M + p] = 0.L;
+    for (int s = p + 1; s <= q; ++s) {
+      orc_ld r2 = 0.L;
+      for (int c = 0; c < d; ++c) { orc_ld df = x[p * d + c] - x[s * d + c]; r2 += df * df; }
+      const orc_ld dist = sqrtl(r2);
+      orc_ld c0 = orc_cov_ld(cov_type, dist, var, range);
+      const orc_ld dd = orc_cov_ddist_ld(cov_type, dist, var, range);
+      const orc_ld g1 = orc_cov_grad_range_ld(cov_type, dist, var, range);
+      G0[p * M + s] = G0[s * M + p] = c0;
+      G1[p * M + s] = G1[s * M + p] = g1;
+      if (F1) {
+        F1[p * M + s] = F1[s * M + p] =
+            u * (cg * fabsl(g1) + fabsl(orc_cov_grad_range_ddist_ld(cov_type, dist, var, range)) *
+                                      (cr * dist + sqrtl((orc_ld)d) * (xn[p] + xn[s])));
+        if (g1 != 0.L) rho1 = fmaxl(rho1, F1[p * M + s] / fabsl(g1));
+      }
+      c0 *= mult;
+      if (drop && drop[0] == r && ((drop[1] == p && drop[2] == s) || (drop[1] == s && drop[2] == p))) c0 = 0.L;
+      St[p * M + s] = St[s * M + p] = c0;
+      E[p * M + s] = E[s * M + p] =
+          u * (cv * fabsl(c0) + fabsl(dd) * (cr * dist + sqrtl((orc_ld)d) * (xn[p] + xn[s])));
+      if (c0 != 0.L) rho = fmaxl(rho, E[p * M + s] / fabsl(c0));
+      orc_ld pre[2];
+      if (efloor > 0.L && orc_exp_arg_ld(cov_type, dist, var, range, pre) > 700.L) {
+        E[p * M + s] = E[s * M + p] = E[p * M + s] + efloor * fabsl(pre[0]);
+        if (F1) F1[p * M + s] = F1[s * M + p] = F1[p * M + s] + efloor * fabsl(pre[1]);
+      }
+    }
+  }
+  *rho_out = rho;
+  if (rho1_out) *rho1_out = rho1;
+  return q;
 }
 
 int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int32_t* nn, int cov_type, double var_d,
@@ -666,40 +758,9 @@ int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int
       const int32_t* nb = nn + (size_t)r * m;
       double* o = out + (size_t)r * ORC_ROWS_NOUT;
       for (int k = 0; k < m; ++k) { A[(size_t)r * m + k] = 0.; bA[(size_t)r * m + k] = 0.; }
-      int q = 0;
-      for (int k = 0; k < m; ++k)
-        if (nb[k] >= 0) pos[q++] = k;
-      for (int c = 0; c < d; ++c) {
-        for (int j = 0; j < q; ++j) x[j * d + c] = coords[(size_t)c * n + nb[pos[j]]];
-        x[q * d + c] = qcoords ? qcoords[(size_t)c * nrows + r] : coords[(size_t)c * n + i];
-      }
-      for (int j = 0; j <= q; ++j) {
-        orc_ld mx = 0.L;
-        for (int c = 0; c < d; ++c) mx = fmaxl(mx, fabsl(x[j * d + c]));
-        xn[j] = mx;
-        yn[j] = j < q ? (orc_ld)y[nb[pos[j]]] : (qcoords ? 0.L : (orc_ld)y[i]);
-      }
-      orc_ld rho = 0.L; /* largest relative evaluation error of one covariance */
-      for (int p = 0; p <= q; ++p) {
-        St[p * M + p] = p < q ? (orc_ld)diag_nb : (orc_ld)diag_obs;
-        G0[p * M + p] = var;
-        G1[p * M + p] = 0.L;
-        for (int s = p + 1; s <= q; ++s) {
-          orc_ld r2 = 0.L;
-          for (int c = 0; c < d; ++c) { orc_ld df = x[p * d + c] - x[s * d + c]; r2 += df * df; }
-          const orc_ld dist = sqrtl(r2);
-          orc_ld c0 = orc_cov_ld(cov_type, dist, var, range);
-          const orc_ld dd = orc_cov_ddist_ld(cov_type, dist, var, range);
-          G0[p * M + s] = G0[s * M + p] = c0;
-          G1[p * M + s] = G1[s * M + p] = orc_cov_grad_range_ld(cov_type, dist, var, range);
-          c0 *= mult;
-          if (drop && drop[0] == r && ((drop[1] == p && drop[2] == s) || (drop[1] == s && drop[2] == p))) c0 = 0.L;
-          St[p * M + s] = St[s * M + p] = c0;
-          E[p * M + s] = E[s * M + p] =
-              u * (cv * fabsl(c0) + fabsl(dd) * (cr * dist + sqrtl((orc_ld)d) * (xn[p] + xn[s])));
-          if (c0 != 0.L) rho = fmaxl(rho, E[p * M + s] / fabsl(c0));
-        }
-      }
+      orc_ld rho; /* largest relative evaluation error of one covariance */
+      const int q = orc_row_build_ld(coords, n, d, m, nb, cov_type, var, range, diag_nb, diag_obs, y, qcoords, i, r, nrows, cv, cr, mult,
+                                     drop, 0.L, pos, x, xn, yn, St, E, G0, G1, NULL, 0.L, &rho, NULL);
       orc_row_ld rw;
       if (orc_row_factor_ld(q, M, u, St, E, yn, L, Si, a, w, t, &rw) != 0) {
         ++bad;
@@ -721,13 +782,143 @@ int orc_vecchia_rows_ld(const double* coords, int64_t n, int d, int m, const int
       o[15] = (double)(bD / D + u * (1.L + fabsl(logl(D))));
       o[22] = (double)rw.kap; o[23] = (double)rw.eps;
       for (int k = 0; k < 2; ++k) {
-        orc_ld g6[6];
+        orc_ld g6[8];
         orc_row_grad_ld(k == 0 ? G0 : G1, q, M, a, w, &rw, ke, g6);
         o[5 + k] = (double)g6[0]; o[7 + k] = (double)g6[1]; o[9 + k] = (double)g6[2];
         o[16 + k] = (double)g6[3]; o[18 + k] = (double)g6[4]; o[20 + k] = (double)g6[5];
       }
     }
     free(x); free(xn); free(St); free(E); free(G0); free(G1); free(L); free(Si); free(a); free(w); free(yn); free(t); free(pos);
+  }
+  return bad;
+}
+
+/* ---- long-double reference of the factor derivatives (MODE_STORE_GRAD / MODE_STORE_GRAD2), rows [row_begin, row_begin + nrows)
+ *
+ * Rows, St, E and the derivative matrices as orc_vecchia_rows_ld (diag_nb / diag_obs: var + 1 twice for the Gaussian factor,
+ * var (1 + 1e-10) and var for the latent one): G0 = Sigma~ - I (diagonal var) for k = 0 (log var), G1 = d Sigma / d log range (zero
+ * diagonal) for k = 1. With b = [-A_i, 1], r_k = the first q entries of G_k b = g_k - G_k,NN A_i (g_k = G_k,Nq):
+ *   dA_k = S_NN^-1 r_k        dD_k = b^T G_k b = G_k,qq - 2 A_i.g_k + A_i^T G_k,NN A_i
+ * by this generic formula for both parameters (the device's variance shortcut S^-1 A, D - 1 - A.A is what it checks).
+ *
+ * First-order bounds of an fp64 evaluation. One forms S_NN + dS (|dS| <= E_NN, which holds the Cholesky backward error), A + dA
+ * (|dA| <= beta_A = |S_NN^-1| (E_N. |b|), as in orc_vecchia_rows_ld), G_k + dG_k (|dG_k| <= F_k), rounds the product G_k b
+ * (gam(q + 2) |G_k| |b|) and solves with the Cholesky factor: the forward and back substitution add a backward error
+ * 2 gam(q + 2) |L| |L^T| <= 2 gam(q + 2) sqrt(S_aa S_bb). To first order
+ *   |dA_k^ - dA_k| <= |S_NN^-1| [ (E_NN + 2 gam(q + 2) sqrt(S_aa S_bb)) |dA_k| + (F_k + gam(q + 2) |G_k|) |b| + |G_k,NN| beta_A ]_N
+ * F_0 is E's evaluation part off the diagonal (covariance evaluation, distance rounding, rounding of the coordinates) and u var on
+ * it; F_1 holds the evaluation errors of the range derivative,
+ *   F1_ab = u (cg |G1_ab| + |dG1/dr|_ab (cr r_ab + sqrt(d) (|x_a|_inf + |x_b|_inf)))
+ * with cg the relative error of its closed form in units of u. Where a pair's exponent exceeds 700, E_ab and F_ab also take exp_floor
+ * times the factor in front of the exp: an fp64 exp(-x) that saturates at exp_floor (the kernels' does, at exp(-700)) is off by up
+ * to that much in absolute terms, far below the fp64 range of the true value. dD_k takes kappa (eps + rho_k) times its magnitude with every factor
+ * in absolute value (orc_row_grad_ld), rho_0 = the rho of orc_vecchia_rows_ld, rho_1 = max(rho_0, max F1_ab / |G1_ab|).
+ *
+ * out: nrows x ORC_DF_NOUT, columns  0 D  1 beta_D  2 dD_0  3 its bound  4 dD_1  5 its bound  6 kappa  7 eps  8 rho_0  9 rho_1
+ * dA, bdA: 2 x nrows x m (parameter, row, slot; 0 at -1 slots). Deliberate faults, for tests of the bounds themselves: range_mult
+ * scales every entry of G1; drop = {row, a, b} removes the pair (a, b) from G1 of one row (S_NN intact); g1_diag is put on G1's
+ * neighbour diagonal (the latent jitter leaking into the derivative); g0_shift is added to G0's diagonal (dSigma~ = Sigma~ -
+ * (1 - delta) I: the nugget moving). The bounds are those of the unfaulted matrices. Returns the number of rows whose neighbour
+ * block is not positive definite. */
+#define ORC_DF_NOUT 10
+
+int orc_vecchia_rows_dfactor_ld(const double* coords, int64_t n, int d, int m, const int32_t* nn, int cov_type, double var_d,
+                                double range_d, double diag_nb, double diag_obs, int64_t row_begin, int64_t nrows, double cv, double cr,
+                                double cg, double exp_floor, double range_mult, const int64_t* drop, double g1_diag, double g0_shift, double* out,
+                                double* dA, double* bdA) {
+  const orc_ld u = ldexpl(1.L, -53), var = var_d, range = range_d;
+  const int M = m + 1;
+  int bad = 0;
+#pragma omp parallel
+  {
+    orc_ld* x = (orc_ld*)malloc(sizeof(orc_ld) * M * d);
+    orc_ld* xn = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* St = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* E = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* F0 = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* F1 = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* G0 = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* G1 = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* L = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* Si = (orc_ld*)malloc(sizeof(orc_ld) * M * M);
+    orc_ld* a = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* w = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* yn = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* t = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* ba = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* rk = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    orc_ld* v = (orc_ld*)malloc(sizeof(orc_ld) * M);
+    int* pos = (int*)malloc(sizeof(int) * M);
+#pragma omp for schedule(dynamic, 64) reduction(+ : bad)
+    for (int64_t r = 0; r < nrows; ++r) {
+      const int64_t i = row_begin + r;
+      const int32_t* nb = nn + (size_t)r * m;
+      double* o = out + (size_t)r * ORC_DF_NOUT;
+      for (int k = 0; k < 2; ++k)
+        for (int s = 0; s < m; ++s) dA[((size_t)k * nrows + r) * m + s] = bdA[((size_t)k * nrows + r) * m + s] = 0.;
+      orc_ld rho0, rho1;
+      const int q = orc_row_build_ld(coords, n, d, m, nb, cov_type, var, range, diag_nb, diag_obs, NULL, NULL, i, r, nrows, cv, cr, 1.L,
+                                     NULL, cg, pos, x, xn, yn, St, E, G0, G1, F1, (orc_ld)exp_floor, &rho0, &rho1);
+      rho1 = fmaxl(rho1, rho0);
+      for (int p = 0; p <= q; ++p) {
+        F0[p * M + p] = u * var;
+        for (int s = 0; s <= q; ++s)
+          if (s != p) F0[p * M + s] = E[p * M + s];
+      }
+      /* deliberate faults */
+      for (int p = 0; p <= q; ++p) {
+        G0[p * M + p] += (orc_ld)g0_shift;
+        if (p < q) G1[p * M + p] = (orc_ld)g1_diag;
+        for (int s = 0; s <= q; ++s) G1[p * M + s] *= (orc_ld)range_mult;
+      }
+      if (drop && drop[0] == r) G1[drop[1] * M + drop[2]] = G1[drop[2] * M + drop[1]] = 0.L;
+      orc_row_ld rw;
+      if (orc_row_factor_ld(q, M, u, St, E, yn, L, Si, a, w, t, &rw) != 0) {
+        ++bad;
+        for (int k = 0; k < ORC_DF_NOUT; ++k) o[k] = NAN;
+        continue;
+      }
+      if (!(rw.D > 0.L)) ++bad;
+      /* a = -b (a[q] = -1), t = E |b|: beta_A */
+      for (int p = 0; p < q; ++p) {
+        orc_ld s = 0.L;
+        for (int c = 0; c < q; ++c) s += fabsl(Si[p * M + c]) * t[c];
+        ba[p] = s;
+      }
+      const orc_ld gam = (q + 2) * u / (1.L - (q + 2) * u);
+      o[0] = (double)rw.D; o[1] = (double)rw.bD; o[6] = (double)rw.kap; o[7] = (double)rw.eps;
+      o[8] = (double)rho0; o[9] = (double)rho1;
+      for (int k = 0; k < 2; ++k) {
+        const orc_ld* G = k == 0 ? G0 : G1;
+        const orc_ld* F = k == 0 ? F0 : F1;
+        for (int p = 0; p < q; ++p) {
+          orc_ld s = 0.L;
+          for (int c = 0; c <= q; ++c) s -= G[p * M + c] * a[c];
+          rk[p] = s;
+        }
+        orc_chol_solve_ld(L, q, M, rk);
+        for (int p = 0; p < q; ++p) {
+          orc_ld s = 0.L;
+          for (int c = 0; c < q; ++c)
+            s += (E[p * M + c] + 2.L * gam * sqrtl(St[p * M + p] * St[c * M + c])) * fabsl(rk[c]) + fabsl(G[p * M + c]) * ba[c];
+          for (int c = 0; c <= q; ++c) s += (F[p * M + c] + gam * fabsl(G[p * M + c])) * fabsl(a[c]);
+          v[p] = s;
+        }
+        for (int p = 0; p < q; ++p) {
+          orc_ld s = 0.L;
+          for (int c = 0; c < q; ++c) s += fabsl(Si[p * M + c]) * v[c];
+          dA[((size_t)k * nrows + r) * m + pos[p]] = (double)rk[p];
+          bdA[((size_t)k * nrows + r) * m + pos[p]] = (double)s;
+        }
+        orc_ld g8[8];
+        const orc_ld ke = rw.kap * (rw.eps + (k == 0 ? rho0 : rho1));
+        orc_row_grad_ld(G, q, M, a, w, &rw, ke, g8);
+        o[2 + 2 * k] = (double)g8[6];
+        o[3 + 2 * k] = (double)(ke * g8[7]);
+      }
+    }
+    free(x); free(xn); free(St); free(E); free(F0); free(F1); free(G0); free(G1); free(L); free(Si); free(a); free(w); free(yn);
+    free(t); free(ba); free(rk); free(v); free(pos);
   }
   return bad;
 }
@@ -850,7 +1041,7 @@ int orc_vecchia_rows_aniso_ld(const double* coords, int64_t n, int d, int m, con
       o[9] = (double)(bD / D + u * (1.L + fabsl(logl(D))));
       o[10] = (double)rw.kap; o[11] = (double)rw.eps;
       for (int k = 0; k < NP; ++k) {
-        orc_ld g6[6];
+        orc_ld g6[8];
         const orc_ld rk = k == 0 ? rho : rho + (orc_ld)share_ulps[k - 1] * u;
         orc_row_grad_ld(G + (size_t)k * M * M, q, M, a, w, &rw, rw.kap * (rw.eps + rk), g6);
         for (int j = 0; j < 3; ++j) {

@@ -35,8 +35,9 @@ The cases reach every dispatch bucket (test_cases_reach_every_dispatch_bucket re
 t in {1, 2, 3, 31, 32, 33, 50, 63, 64, 65, 96, 97, 127, 128} (G = 1 ... 4), m in {1, 2, 5, 15, 16, 17, 29, 30}, n from 2 and
 m + 1 (every row padded) up to 1e5, d in {1, 2, 3, 4} (Morton order at d = 2 and 3, index order at d = 1 and 4), W = 0,
 W in (0, 0.25] and D^-1 spread over several decades, and hand-built neighbour patterns: a chain (depth n - 1, up to n = 1e5), a
-star (column 0 has n - 1 entries), columns of exactly 15, 16, 17, 31, 32, 33, 127, 128 and 129 entries (around trs_bwd's 16-entry
-batches, mv_Bt's 32-entry chunks and v_trs_bwd's 128-entry unrolled loop) and a comb (depth 1: every row depends on the first 30
+star (column 0 has n - 1 entries), columns of exactly 7, 8, 9, 15, 16, 17, 31, 32, 33, 64, 127, 128 and 129 entries (around
+trs_bwd's 16-entry batches, mv_Bt's 32-entry chunks, v_trs_bwd's 128-entry unrolled loop and the 8-row batches of the Fisher
+contraction) and a comb (depth 1: every row depends on the first 30
 rows).
 
 End to end, GPModel at num_rand_vec_trace = t for t in {1, 2, 31, 32, 33, 64, 65, 97, 128} runs against oracle.laplace with the
@@ -58,7 +59,7 @@ LD = np.longdouble
 SENTINEL = 0x7ff8dead0badf00d
 T_ALL = (1, 2, 3, 31, 32, 33, 50, 63, 64, 65, 96, 97, 127, 128)
 OP_NAMES = ("DinvBX", "BtX+WX2", "SigmaI+W", "Pinv", "Bt_inv", "BgX", "X2+BgtX")
-COL_COUNTS = (15, 16, 17, 31, 32, 33, 127, 128, 129)
+COL_COUNTS = (7, 8, 9, 15, 16, 17, 31, 32, 33, 64, 127, 128, 129)
 WORST = {}  # op name -> worst error / bar ratio seen in this session
 
 
@@ -85,7 +86,7 @@ def star_nn(n, m):
 
 
 def colcount_nn(n):
-    """columns 0 ... 8 have exactly COL_COUNTS entries: one from the row after them (every row also depends on its predecessor),
+    """columns 0 ... 12 have exactly COL_COUNTS entries: one from the row after them (every row also depends on its predecessor),
     the rest from consecutive blocks of later rows"""
     hubs = []
     for h, c in enumerate(COL_COUNTS):
@@ -169,8 +170,8 @@ CASES = [
     ("chain-3000", 3000, 2, 1, "chain", (1, 2, 65), "small", 0),
     ("chain-1e5", 100000, 2, 1, "chain", (1, 50), "small", 0),
     ("star-5000", 5000, 2, 5, "star", (1, 50), "small", 0),
-    ("colcounts", 600, 2, 2, "cols", (1, 3, 33), "small", 0),
-    ("colcounts-index", 600, 4, 2, "cols", (1, 64), "zero", 0),
+    ("colcounts", 700, 2, 2, "cols", (1, 3, 33), "small", 0),
+    ("colcounts-index", 700, 4, 2, "cols", (1, 64), "zero", 0),
     ("comb-3000", 3000, 2, 30, "comb", (1, 64), "small", 0),
 ]
 CASE_T = [(c, t) for c in CASES for t in c[5]]
@@ -621,11 +622,11 @@ def test_engineered_patterns_have_the_advertised_shape():
         assert depth(chain_nn(n)) == n - 1
     nn = star_nn(5000, 5)
     assert col_counts(nn)[0] == 4999 and depth(nn) == 4999
-    cc = col_counts(colcount_nn(600))
+    cc = col_counts(colcount_nn(700))
     assert list(cc[:len(COL_COUNTS)]) == list(COL_COUNTS) and set(cc[len(COL_COUNTS):]) <= {0, 1}
     nn = comb_nn(3000)
     assert depth(nn) == 1 and np.all(col_counts(nn)[:30] == 2970) and np.all(col_counts(nn)[30:] == 0)
-    for nn in (chain_nn(50), star_nn(50, 5), colcount_nn(600), comb_nn(100)):
+    for nn in (chain_nn(50), star_nn(50, 5), colcount_nn(700), comb_nn(100)):
         for i in range(nn.shape[0]):
             r = nn[i][nn[i] >= 0]
             assert np.all(r < i) and len(set(r)) == r.size

@@ -126,7 +126,8 @@ def reference(co, nn, cid, pt, y_ord, row_begin=0, row_end=None, **faults):
 
 # ---------------------------------------------------------------------------------------------------------- CPU-only
 def mp_rows(co, nn, cid, var, rng_, diag_nb, diag_obs, y, rows, qcoords=None):
-    """the same row quantities with mpmath at 50 digits"""
+    """the same row quantities with mpmath at 50 digits; "dA" and "dD" hold the factor derivatives w.r.t. log var (k = 0,
+    dSigma~ = Sigma~ - I) and log range (k = 1): dA_k = S^-1 (g_k - G_k A), dD_k = G_k,qq - 2 A.g_k + A^T G_k A"""
     mp = pytest.importorskip("mpmath")
     mp.mp.dps = 50
     var, rng_ = mp.mpf(var), mp.mpf(rng_)
@@ -155,7 +156,7 @@ def mp_rows(co, nn, cid, var, rng_, diag_nb, diag_obs, y, rows, qcoords=None):
         dist = lambda a, b: mp.sqrt(sum((a[k] - b[k]) ** 2 for k in range(len(a))))
         D = mp.mpf(diag_obs)
         By = yi
-        out = {"A": [], "t": [mp.mpf(0)] * 6}
+        out = {"A": [], "t": [mp.mpf(0)] * 6, "dA": [[], []], "dD": [var, mp.mpf(0)]}
         if q == 0:
             u = By / D
             out.update(D=D, By=By)
@@ -186,6 +187,9 @@ def mp_rows(co, nn, cid, var, rng_, diag_nb, diag_obs, y, rows, qcoords=None):
             uk = -sum((g[k][a] - GA[a]) * w[a] for a in range(q))
             dD = (var if k == 0 else 0) - 2 * sum(A[a] * g[k][a] for a in range(q)) + sum(A[a] * GA[a] for a in range(q))
             t.append((uk * u, u * u * dD, dD / D))
+            dAk = mp.lu_solve(S, g[k] - GA)
+            out["dA"][k] = [dAk[a] for a in range(q)]
+            out["dD"][k] = dD
         out.update(D=D, By=By, A=[A[k] for k in range(q)], t=[t[0][0], t[1][0], t[0][1], t[1][1], t[0][2], t[1][2]])
         res.append(out)
     return res
